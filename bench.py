@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — YUME denoise-step benchmark on B200 (driver contract: one JSON line on stdout from rank 0).
+"""bench.py — YUME denoise-step benchmark on H100 (one JSON result line on stdout from rank 0).
 
 Workload at N=1 = BASELINE.json configs[1]: one Yume-5B-720P denoise step (WanModel.forward, wan23 tree) on an
 81-frame 704x1280 latent [48,21,44,80] -> L = 18 480 tokens, random-init bf16-valued weights, synthetic Gaussian
@@ -9,15 +9,19 @@ is the denoise-step latency BASELINE.json names).
   value      device-resident inputs (latent, t, context already in HBM), CUDA-event timed
   e2e        the same step through the reference-facing `WanModel.forward(x, t, context, seq_len, flag=False)`
              with pinned HOST inputs: H2D copies and the D2H read of the result are inside the timed region
-  roofline   the dominant kernel (self-attention, attention_kernel<true>) timed live with CUDA events on the
+  roofline   the dominant kernel (self-attention, attention_kernel<false>) timed live with CUDA events on the
              launching stream inside the timed steps: achieved = 4*L^2*C FLOP / mean launch time
   cpu_baseline / --impl reference: the oracle port of the reference forward (oracle/wan_dit.py) on the host cores,
              on a bounded sample (one WanAttentionBlock of the same workload, extrapolated by FLOPs).
 N > 1: Ulysses sequence parallelism over NCCL (one process per GPU, torchrun) — strong scaling of the same step.
+--dump-outputs DIR: after the timed steps, the output of the last timed step is written as DIR/<name>.npy (float32, at most
+64 MB in all; a larger output is replaced by a fixed, seeded sample of its elements). Inputs and weights are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
 import argparse
+import gc
 import json
 import math
 import os
@@ -44,14 +48,16 @@ def block_flops(L: int, C: int, F: int, S: int) -> float:
     return 8 * L * C * C + 4 * L * L * C + 4 * L * C * C + 4 * S * C * C + 4 * L * S * C + 4 * L * C * F
 
 
-def synthetic_state_dict(cfg: dict, device, seed: int = 0):
+def synthetic_state_dict(cfg: dict, device, seed: int = 0, dtype=torch.float32):
     """Random-init weights with the reference's state-dict keys, generated on the device, bf16-representable
-    (the reference zero-inits head.head — model.py:914 — which would make the output 0; we use N(0, 0.02))."""
+    (the reference zero-inits head.head — model.py:914 — which would make the output 0; we use N(0, 0.02)).
+    dtype = torch.bfloat16 stores the same values in half the memory (the 14B weights do not fit an 80 GB GPU twice in fp32);
+    the 1 + N(0, 0.1) norm weights stay fp32 in either case."""
     g = torch.Generator(device=device).manual_seed(seed)
     C, Fd, cin, cout = cfg["dim"], cfg["ffn_dim"], cfg["in_dim"], cfg["out_dim"]
 
     def rn(*shape, std=1.0):
-        return (torch.randn(*shape, generator=g, device=device) * std).to(torch.bfloat16).to(torch.float32)
+        return (torch.randn(*shape, generator=g, device=device) * std).to(torch.bfloat16).to(dtype)
 
     sd = {}
     for name, k in (("patch_embedding", 2), ("patch_embedding_2x", 4), ("patch_embedding_4x", 8),
@@ -68,20 +74,20 @@ def synthetic_state_dict(cfg: dict, device, seed: int = 0):
     img = cfg["variant"] == "14b"
     if img:
         cd = cfg["clip_dim"]
-        sd["img_emb.proj.0.weight"], sd["img_emb.proj.0.bias"] = 1 + rn(cd, std=0.1), rn(cd, std=0.02)
+        sd["img_emb.proj.0.weight"], sd["img_emb.proj.0.bias"] = 1 + rn(cd, std=0.1).float(), rn(cd, std=0.02)
         sd["img_emb.proj.1.weight"], sd["img_emb.proj.1.bias"] = rn(cd, cd, std=cd ** -0.5), rn(cd, std=0.02)
         sd["img_emb.proj.3.weight"], sd["img_emb.proj.3.bias"] = rn(C, cd, std=cd ** -0.5), rn(C, std=0.02)
-        sd["img_emb.proj.4.weight"], sd["img_emb.proj.4.bias"] = 1 + rn(C, std=0.1), rn(C, std=0.02)
+        sd["img_emb.proj.4.weight"], sd["img_emb.proj.4.bias"] = 1 + rn(C, std=0.1).float(), rn(C, std=0.02)
     for i in range(cfg["num_layers"]):
         p = f"blocks.{i}"
         for att in ("self_attn", "cross_attn"):
             for pr in ("q", "k", "v", "o") + (("k_img", "v_img") if (img and att == "cross_attn") else ()):
                 sd[f"{p}.{att}.{pr}.weight"], sd[f"{p}.{att}.{pr}.bias"] = rn(C, C, std=C ** -0.5), rn(C, std=0.02)
-            sd[f"{p}.{att}.norm_q.weight"] = 1 + rn(C, std=0.1)
-            sd[f"{p}.{att}.norm_k.weight"] = 1 + rn(C, std=0.1)
+            sd[f"{p}.{att}.norm_q.weight"] = 1 + rn(C, std=0.1).float()
+            sd[f"{p}.{att}.norm_k.weight"] = 1 + rn(C, std=0.1).float()
             if img and att == "cross_attn":
-                sd[f"{p}.{att}.norm_k_img.weight"] = 1 + rn(C, std=0.1)
-        sd[f"{p}.norm3.weight"], sd[f"{p}.norm3.bias"] = 1 + rn(C, std=0.1), rn(C, std=0.02)
+                sd[f"{p}.{att}.norm_k_img.weight"] = 1 + rn(C, std=0.1).float()
+        sd[f"{p}.norm3.weight"], sd[f"{p}.norm3.bias"] = 1 + rn(C, std=0.1).float(), rn(C, std=0.02)
         sd[f"{p}.ffn.0.weight"], sd[f"{p}.ffn.0.bias"] = rn(Fd, C, std=C ** -0.5), rn(Fd, std=0.02)
         sd[f"{p}.ffn.2.weight"], sd[f"{p}.ffn.2.bias"] = rn(C, Fd, std=Fd ** -0.5), rn(C, std=0.02)
         sd[f"{p}.modulation"] = rn(1, 6, C, std=C ** -0.5)
@@ -96,7 +102,7 @@ def measured_peaks():
         d = json.loads(f.read_text())
         return dict(hbm_gbs=d["hbm_gbs"], bf16_tflops=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained"),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_sustained=None, source="H100 SXM data sheet (dense bf16, 700 W card)")
 
 
 # ------------------------------------------------------------------------------------------------------------
@@ -189,12 +195,12 @@ def reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------------------------------
-# GPU comparator: the reference's own eager regime (PyTorch ops + SDPA under autocast bf16) on the same B200
+# GPU comparator: the reference's own eager regime (PyTorch ops + SDPA under autocast bf16) on the same GPU
 # ------------------------------------------------------------------------------------------------------------
 def gpu_comparator(dev):
     """The oracle port of WanAttentionBlock.forward run ON THE GPU the way the reference runs its model: stock PyTorch
     eager kernels under torch.autocast(bf16), attention through F.scaled_dot_product_attention (the library FMHA; the
-    reference calls flash_attn, absent here — SDPA is the faster of the two on sm_100, profiles/README.md), RoPE in
+    reference calls flash_attn, which is not installed here), RoPE in
     complex128 as the reference does. One block at the full L = 18 480, x 30 blocks. BASELINE.md §4."""
     from oracle import synth
     from oracle.wan_dit import WanOracle, grid_freqs
@@ -340,15 +346,16 @@ def supplementary(args, dev, eng5, world, rank, peaks):
         e5.use_cuda_graph = False
     out["5b-chunk-4step"]["config"] = ("BASELINE configs[3]: sample_5b.py:941-1034 loop, 4 Euler steps shift 7.0, L=9460 (5 history "
                                        "+ 8 new latent frames @44x80), per-token t; context K/V cached across the steps")
-    # free the 5B engine before the 14B one is built
+    # free the 5B engine before the 14B one is built (install() binds forward on the module: a reference cycle, hence gc.collect)
     eng5.clear()
     del model5, e5
+    gc.collect()
     torch.cuda.empty_cache()
 
     # ---- configs[2]: Yume-I2V-540P (14B): one FramePack-chunk forward, and a 5-step slice of the 50-step CFG ODE ----
     if not args.no_14b:
         cfg = CFG_14B
-        sd = synthetic_state_dict(cfg, dev, seed=0)
+        sd = synthetic_state_dict(cfg, dev, seed=0, dtype=torch.bfloat16)
         with torch.device("meta"):
             m14 = WanModel14B(model_type="i2v", text_len=cfg["text_len"], in_dim=cfg["in_dim"], dim=cfg["dim"],
                               ffn_dim=cfg["ffn_dim"], freq_dim=cfg["freq_dim"], text_dim=cfg["text_dim"],
@@ -396,6 +403,7 @@ def supplementary(args, dev, eng5, world, rank, peaks):
         except Exception as e:   # never lose the other entries to the largest one
             out["14b-grid-81f"] = {"error": f"{type(e).__name__}: {e}"[:500]}
         del m14, e14
+        gc.collect()
         torch.cuda.empty_cache()
 
     # ---- VAE decodes (one GPU) ----
@@ -408,7 +416,13 @@ def supplementary(args, dev, eng5, world, rank, peaks):
         from yume_b200.vae22 import decoder_param_shapes as v22_shapes
 
         def vae_entry(name, eng, z, frames_of, config, encode=False):
-            ms, clocks, launches, tflop, res = _timed_simple((lambda: eng.encode(z)) if encode else (lambda: eng.decode(z)), 2, 1, li)
+            try:
+                ms, clocks, launches, tflop, res = _timed_simple((lambda: eng.encode(z)) if encode else (lambda: eng.decode(z)), 2, 1, li)
+            except torch.cuda.OutOfMemoryError as e:   # an entry too large for this GPU costs only itself, loudly
+                out[name] = {"error": f"{type(e).__name__}: {e}"[:300], "config": config}
+                print(f"bench.py: supplementary entry {name} ran out of device memory: {e}", file=sys.stderr, flush=True)
+                torch.cuda.empty_cache()
+                return
             frames = frames_of(res)
             out[name] = {"ms_per_decode": ms, "value": frames / (ms * 1e-3), "unit": ("encoded" if encode else "decoded") + " frames/s",
                          "frames": frames,
@@ -426,23 +440,25 @@ def supplementary(args, dev, eng5, world, rank, peaks):
                   "BASELINE configs[4]: hyvideo AutoencoderKLCausal3D tiled decode z[1,16,21,90,160] -> [1,3,81,720,1280], 56 tiles")
         del hy
         v22 = Wan22VaeDecoder(_rand_sd(v22_shapes(), dev), device=dev)
-        vae_entry("vae22", v22, torch.randn(48, 21, 44, 80, generator=g, device=dev), lambda r: r.shape[1],
-                  "Wan2.2 VAE one-pass decode z[48,21,44,80] -> [3,81,704,1280] (what sample_5b.py decodes with)")
+        # the Wan VAEs run one FramePack chunk (13 latent frames = 49 video frames): the one-pass 81-frame 720p decode needs more
+        # than the 80 GB of an H100
+        vae_entry("vae22", v22, torch.randn(48, 13, 44, 80, generator=g, device=dev), lambda r: r.shape[1],
+                  "Wan2.2 VAE one-pass decode z[48,13,44,80] -> [3,49,704,1280] (what sample_5b.py decodes with)")
         del v22
         v21 = Wan21VaeDecoder(_rand_sd(v21_shapes(), dev), device=dev)
-        vae_entry("vae21", v21, torch.randn(16, 21, 68, 120, generator=g, device=dev), lambda r: r.shape[1],
-                  "Wan2.1 VAE one-pass decode z[16,21,68,120] -> [3,81,544,960] (what sample.py decodes with)")
+        vae_entry("vae21", v21, torch.randn(16, 13, 68, 120, generator=g, device=dev), lambda r: r.shape[1],
+                  "Wan2.1 VAE one-pass decode z[16,13,68,120] -> [3,49,544,960] (what sample.py decodes with)")
         del v21
         torch.cuda.empty_cache()
         # ---- VAE encodes (SURVEY.md §8(f) rank 3): the history / first-frame conditioning encodes of the two samplers ----
         from yume_b200.vae_enc import Wan21VaeEncoder, Wan22VaeEncoder, encoder_param_shapes_21, encoder_param_shapes_22
         e22 = Wan22VaeEncoder(_rand_sd(encoder_param_shapes_22(), dev), device=dev)
-        vae_entry("vae22-encode", e22, torch.randn(3, 81, 704, 1280, generator=g, device=dev).clamp_(-1, 1), lambda r: 81,
-                  "Wan2.2 VAE one-pass encode video[3,81,704,1280] -> mu[48,21,44,80] (sample_5b.py:892-893 history encode)", encode=True)
+        vae_entry("vae22-encode", e22, torch.randn(3, 49, 704, 1280, generator=g, device=dev).clamp_(-1, 1), lambda r: 49,
+                  "Wan2.2 VAE one-pass encode video[3,49,704,1280] -> mu[48,13,44,80] (sample_5b.py:892-893 history encode)", encode=True)
         del e22
         e21 = Wan21VaeEncoder(_rand_sd(encoder_param_shapes_21(), dev), device=dev)
-        vae_entry("vae21-encode", e21, torch.randn(3, 81, 544, 960, generator=g, device=dev).clamp_(-1, 1), lambda r: 81,
-                  "Wan2.1 VAE one-pass encode video[3,81,544,960] -> mu[16,21,68,120] (wan/image2video.py:348-367 conditioning encode)",
+        vae_entry("vae21-encode", e21, torch.randn(3, 49, 544, 960, generator=g, device=dev).clamp_(-1, 1), lambda r: 49,
+                  "Wan2.1 VAE one-pass encode video[3,49,544,960] -> mu[16,13,68,120] (wan/image2video.py:348-367 conditioning encode)",
                   encode=True)
         del e21
         torch.cuda.empty_cache()
@@ -504,12 +520,14 @@ def product_arm(args):
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}
+
     def timed(fn, steps):
         barrier()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(steps):
-            fn()
+            last["out"] = fn()
         e1.record()
         barrier()
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev)
@@ -527,6 +545,8 @@ def product_arm(args):
         ops.reset_launch_count()
         total_ms = timed(step_device, args.steps)
         launches = ops.launch_count()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"latent_out": last["out"]})
     # ---- e2e: the same step through the reference-facing WanModel.forward with pinned HOST tensors ----
     if args.quick:
         e2e_ms = float("nan")
@@ -572,16 +592,9 @@ def product_arm(args):
     if att:
         ach = att_flops / (att["mean_ms"] * 1e-3) / 1e12
         peak = peaks["bf16_sustained"] or peaks["bf16_tflops"]
-        traffic, traffic_src = None, None
-        tf = ROOT / "profiles" / "r02_attention_traffic.json"
-        if world == 1 and tf.exists():
-            tj = json.loads(tf.read_text())
-            traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
         roof = {"bound": "tensor", "kernel": "yb::attention kernel (self-attention launch)", "achieved": ach, "peak": peak,
                 "unit": "TFLOP/s", "frac": ach / peak,
-                "traffic": traffic, "traffic_unit": "bytes/launch",
-                "traffic_source": traffic_src or "none this run (offline `ncu --set full` capture; see profiles/)",
-                "peak_source": peaks["source"] + ", sustained cuBLAS bf16 (kernel timed inside a long step)",
+                "traffic": None, "peak_source": peaks["source"],
                 "mean_launch_ms": att["mean_ms"], "launches_timed": att["count"],
                 "share_of_step": att["total_ms"] / instr_ms,
                 "timing": f"CUDA events around each launch in a separate {k_steps}-step instrumented pass "
@@ -610,7 +623,7 @@ def product_arm(args):
                        "parallelism": "single GPU" if world == 1 else
                        f"ulysses sp{world} (transport {eng.sp_transport}: "
                        f"{'NVLink peer-memory exchange fused into kernels' if eng._sp_p2p else 'NCCL all-to-all'})",
-                       "l2": "per-step working set (10 GB of bf16 weights + 1.5 GB activations) >> 126 MB L2; no flush needed",
+                       "l2": "per-step working set (10 GB of bf16 weights + 1.5 GB activations) >> 50 MB L2; no flush needed",
                        "caching": "none: text embedding and all 30 cross-attention K/V projections are recomputed inside every timed step",
                        "step_tflop": step_flops / 1e12},
             "step_tflops_achieved": step_flops / (ms_per_step * 1e-3) / 1e12,
@@ -658,7 +671,7 @@ def chunk_arm(args):
     torch.cuda.set_device(0)
     five = args.config == "5b-chunk"
     cfg = CFG_5B if five else CFG_14B
-    sd = synthetic_state_dict(cfg, dev, seed=0)
+    sd = synthetic_state_dict(cfg, dev, seed=0, dtype=torch.float32 if five else torch.bfloat16)
     kw = {k: cfg[k] for k in ("dim", "ffn_dim", "num_heads", "num_layers", "in_dim", "out_dim", "text_len", "freq_dim")}
     eng = WanDiT(sd, cfg["variant"], device=dev, **kw)
     del sd
@@ -687,6 +700,8 @@ def chunk_arm(args):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"latent_out": out})
     flops = cfg["num_layers"] * block_flops(L, cfg["dim"], cfg["ffn_dim"], S)
     print(json.dumps({"metric": "latent_frames_per_sec", "value": 8 / (ms * 1e-3), "unit": "latent-frames/s", "n_gpus": 1,
                       "steps": args.steps, "warmup": max(3, args.warmup), "ms_per_step": ms, "higher_is_better": True,
@@ -733,6 +748,8 @@ def vae_arm(args):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"video_out": out})
     frames = out.shape[2]
     print(json.dumps({"metric": "decoded_frames_per_sec", "value": frames / (ms * 1e-3), "unit": "frames/s", "n_gpus": 1,
                       "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
@@ -744,15 +761,16 @@ def vae_arm(args):
 
 def vae22_arm(args):
     """Supplementary workloads (SURVEY.md §8(f) rank 1), random-init weights at the real widths:
-    vae22 — Wan2.2 VAE decode of the 5B sampler's latent z [48,21,44,80] -> video [3,81,704,1280] (`Wan2_2_VAE.decode`);
-    vae21 — Wan2.1 VAE decode of the 14B sampler's 540p latent z [16,21,68,120] -> [3,81,544,960] (`WanVAE.decode`)."""
+    vae22 — Wan2.2 VAE decode of one 5B FramePack chunk z [48,13,44,80] -> video [3,49,704,1280] (`Wan2_2_VAE.decode`);
+    vae21 — Wan2.1 VAE decode of one 14B 540p chunk z [16,13,68,120] -> [3,49,544,960] (`WanVAE.decode`).
+    The one-pass 81-frame decode needs more than the 80 GB of an H100."""
     from yume_b200 import ops
     if args.workload == "vae22":
         from yume_b200.vae22 import Wan22VaeDecoder as Decoder, decoder_param_shapes
-        zc, full, label = 48, (21, 44, 80), "Wan2.2 VAE"
+        zc, full, label = 48, (13, 44, 80), "Wan2.2 VAE"
     else:
         from yume_b200.vae21 import Wan21VaeDecoder as Decoder, decoder_param_shapes
-        zc, full, label = 16, (21, 68, 120), "Wan2.1 VAE"
+        zc, full, label = 16, (13, 68, 120), "Wan2.1 VAE"
 
     dev = torch.device("cuda", 0)
     torch.cuda.set_device(0)
@@ -781,12 +799,33 @@ def vae22_arm(args):
     e1.record()
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / args.steps
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, {"video_out": out})
     print(json.dumps({"metric": "decoded_frames_per_sec", "value": out.shape[1] / (ms * 1e-3), "unit": "frames/s", "n_gpus": 1,
                       "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
                       "dtype": "bf16", "data": "synthetic",
                       "config": {"workload": f"{label} whole-sequence decode z[{zc},{T},{H},{W}] -> {tuple(out.shape)}"},
                       "gpu_launches": ops.launch_count(), "peak_mem_gb": torch.cuda.max_memory_allocated() / 2**30,
                       "finite": bool(torch.isfinite(out).all())}), flush=True)
+
+
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(dirname, arrays: dict):
+    """Writes each tensor as DIR/<name>.npy in float32. A tensor larger than its share of DUMP_BYTES is replaced by a fixed
+    sample of its flattened elements: indices drawn from a generator seeded with 0, in ascending order, so the same shape gives
+    the same positions in every run."""
+    import numpy as np
+    d = Path(dirname)
+    d.mkdir(parents=True, exist_ok=True)
+    share = DUMP_BYTES // (4 * len(arrays))
+    for name, t in arrays.items():
+        arr = t.detach().float().cpu()
+        if arr.numel() > share:
+            idx = torch.randint(0, arr.numel(), (share,), generator=torch.Generator().manual_seed(0)).sort().values
+            arr = arr.reshape(-1)[idx]
+        np.save(d / f"{name}.npy", arr.numpy())
 
 
 def main():
@@ -803,8 +842,9 @@ def main():
     ap.add_argument("--no-14b", action="store_true", help="supplementary: skip the 14B runs")
     ap.add_argument("--no-vae", action="store_true", help="supplementary: skip the VAE decodes")
     ap.add_argument("--sp-transport", default="auto", choices=["auto", "p2p", "p2p_gemm", "nccl"])
-    ap.add_argument("--gemm-split-k", type=int, default=0, choices=[0, 1], help="tail split-K of the gate+residual GEMMs: 0 automatic, 1 never (A/B)")
+    ap.add_argument("--gemm-split-k", type=int, default=0, choices=[0, 1], help="tail split-K of SM-pair gate+residual GEMMs: 0 automatic, 1 never; the default path uses no SM-pair GEMM")
     ap.add_argument("--quick", action="store_true", help="profiling runs: exact --warmup, no e2e leg, no CPU baseline")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the output of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.gemm_split_k:
         from yume_b200 import ops as _ops

@@ -1,4 +1,4 @@
-/* yume_b200.h — C ABI of libyume_b200.so: the B200 (sm_100a) kernels behind YUME's denoise hot path.
+/* yume_b200.h — C ABI of libyume_b200.so: the H100 (sm_90a) kernels behind YUME's denoise hot path.
  *
  * The reference (stdstu12/YUME) has no FFI: its extension seam is Python method re-binding on the
  * WanModel instance (wan23/textimage2video.py:190-194) plus the module-level function
@@ -29,7 +29,7 @@ extern "C" {
 int yb_abi_version(void);
 
 /* ---------------------------------------------------------------------------------------------
- * GEMM with fused epilogue: out = epi(A[M,K] * B[N,K]^T + bias[N]); A, B bf16; fp32 accumulate (tcgen05).
+ * GEMM with fused epilogue: out = epi(A[M,K] * B[N,K]^T + bias[N]); A, B bf16; fp32 accumulate (wgmma).
  * Replaces nn.Linear q/k/v/o (wan23/modules/model.py:171-174,190-192,206), ffn (:265-267,309-312),
  * text_embedding (:455-457), cross-attn projections (:222-224,231) and the patch-embedding Conv3d
  * (kernel==stride, :453-454) after yb_patchify has gathered the patches.
@@ -45,8 +45,8 @@ int yb_abi_version(void);
 
 typedef struct yb_gemm_args {
   unsigned int struct_bytes; /* = sizeof(yb_gemm_args): the library rejects a caller built against another layout */
-  int cta_pair;    /* kernel choice: 0 = automatic (SM-pair `cta_group::2` kernel for M >= 1024 token GEMMs, 1-CTA kernel for the small
-                      context / embedding projections), 1 = force the 1-CTA kernel, 2 = force the SM-pair kernel (tests, tuning) */
+  int cta_pair;    /* kernel choice: 0 = automatic (the 1-CTA kernel: the faster form on the H100, see yb_gemm_plan), 1 = the 1-CTA
+                      kernel, 2 = the SM-pair kernel (a 2-CTA cluster per 256-row tile, B operand multicast) */
   const void* A;   /* bf16 [M, K], row stride lda */
   const void* B;   /* bf16 [N, K], row stride ldb  (nn.Linear.weight layout) */
   const void* bias;/* f32 [N] or NULL */
@@ -56,8 +56,8 @@ typedef struct yb_gemm_args {
   long long lda, ldb, ldo, gate_ld;
   int M, N, K;
   int epilogue;    /* YB_EPI_* */
-  int block_n;     /* N tile: 0 = auto; 1-CTA kernel 128 / 256; SM-pair kernel any multiple of 32 up to 256 (auto: the width that
-                      minimises waves x width on the SM pairs, yb_gemm_plan) */
+  int block_n;     /* N tile: 0 = auto; 1-CTA kernel 128 / 256; SM-pair kernel any multiple of 32 up to 256 (auto: 256, or N rounded
+                      up to 32 when N < 256) */
   int n_split;     /* YB_EPI_BF16 only: > 0 => output column block j (width n_split, % 32 == 0) is written at
                       out + j*split_stride + m*ldo + (n % n_split): the peer-major layout the Ulysses all-to-all sends */
   long long split_stride;
@@ -68,7 +68,7 @@ typedef struct yb_gemm_args {
   const void* res;  /* YB_EPI_RES_BF16: bf16 [M, N] residual, row stride res_ld */
   long long res_ld;
   /* Tail split-K (SM-pair kernel, YB_EPI_GATE_RES): when the last wave of output tiles fills at most part of the SM pairs (the
-   * per-rank shapes of 4- / 8-GPU Ulysses: 228 / 120 tiles on 74 pairs), its tiles are cut into K segments that run as separate work
+   * per-rank shapes of multi-GPU Ulysses), its tiles are cut into K segments that run as separate work
    * items and leave fp32 partials in `ws`; a second kernel adds them and applies the epilogue. split_k: 0 = automatic,
    * 1 = never, 2..12 = force that many segments on the last wave (tests). ws / ws_bytes: CALLER-owned workspace of at least
    * yb_gemm_workspace_bytes(...) bytes, 16-byte aligned; NULL or too small = the launch is simply not split (same result up to
@@ -87,7 +87,7 @@ int yb_gemm_plan(int M, int N, int sms, int* out4);
 
 /* ---------------------------------------------------------------------------------------------
  * CausalConv3d k=3 (replicate pad W 1,1 / H 1,1 / T 2,0 then Conv3d: hyvideo/vae/unet_causal_3d_blocks.py:48-74) as an
- * implicit GEMM on tcgen05: out[voxel, co] = bias[co] + sum_{tap,ci} xpad[t+dt, h+dh, w+dw, ci] * w[co, tap*Cp + ci].
+ * implicit GEMM on wgmma: out[voxel, co] = bias[co] + sum_{tap,ci} xpad[t+dt, h+dh, w+dw, ci] * w[co, tap*Cp + ci].
  *   xpad  bf16 [T+2, H+2, W+2, Cp] channels-last, already replicate-padded (yb_vae_pad_act writes it), Cp % 64 == 0
  *   w     bf16 [Cout, 27*Cp], tap = (dt*3 + dh)*3 + dw (Conv3d weight permuted to [co, kt, kh, kw, ci]); Cout % 32 == 0
  *   out   [T*H*W, ldo] channels-last; epilogue YB_EPI_BF16, YB_EPI_F32 or YB_EPI_RES_BF16 (+ res bf16 [T*H*W, res_ld])
@@ -95,7 +95,7 @@ int yb_gemm_plan(int M, int N, int sms, int* out4);
 typedef struct yb_conv3d_args {
   unsigned int struct_bytes; /* = sizeof(yb_conv3d_args) */
   int cta_pair;              /* SM-pair kernel (each CTA of a cluster owns one 128-voxel box, the weight tile is split between the two,
-                                un-fused taps): 0 = automatic (output widths 192 / 384), 1 = always, 2 = never */
+                                un-fused taps): 1 = always; 0 (automatic) and 2 = the 1-CTA kernel */
   const void* xpad;
   const void* w;
   const void* bias; /* f32 [Cout] or NULL */
@@ -176,15 +176,12 @@ int yb_attention(const void* q, long long ldq, const void* k, long long ldk, con
                  long long ldo, int Lq, int Lk, int heads, float scale, int flags, void* stream);
 /* Full form. `ws` / `ws_bytes`: caller-owned device workspace for the automatic KV tail split (size it with
  * yb_attention_workspace_bytes; NULL or too small = the launch is not split — same result, a partly idle last wave; the
- * library itself never allocates and never synchronises, so the call is CUDA-graph-capture safe). `trace`: optional clock64
- * trace buffer (int64 [32*32]) filled by CTA (1,0) for KV tiles 16..47: per tile
- * [X*8 + {0: before S wait, 1: S ready, 2: S in registers, 3: row max done, 4: P stored, 5: arrived}] for the softmax
- * warp of query tile X, and [16 + X*4 + {0: before P wait, 1: P ready, 2: PV+S issued}] for the MMA thread. Tuning / tests
- * only; pass NULL in production. */
+ * library itself never allocates and never synchronises, so the call is CUDA-graph-capture safe). `trace`: ignored (kept so that
+ * callers built against earlier versions of this header still link); pass NULL. */
 int yb_attention_ex(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
                     long long ldo, int Lq, int Lk, int heads, float scale, int flags, void* ws, long long ws_bytes,
                     void* trace, void* stream);
-#define YB_ATT_P_SMEM 1     /* flags bit 0: stage P through shared memory instead of TMEM (debug variant) */
+#define YB_ATT_P_SMEM 1     /* flags bit 0: stage P through shared memory instead of registers (debug variant) */
 #define YB_ATT_EMU_SHIFT 2  /* flags bits 2-3: retired (FMA-pipe exponentials: measured slower in rounds 1 and 2, removed); must be 0 */
 #define YB_ATT_ACCUMULATE 2 /* flags bit 1: out += result (WanI2VCrossAttention sums the text and image branches,
                                wan/modules/model.py:380-387) */
@@ -214,7 +211,7 @@ int yb_debug_force_split(int ns);
 int yb_sp_scatter_qkv(const void* qkv, long long ld, const void* wq, const void* wk, const void* rope, int rope_len,
                       int L, int C, int D, float eps, void* const* peers, int world, int rank, int Lp, void* stream);
 /* GEMM + collective in ONE kernel (the second Ulysses transport, "p2p_gemm"): the fused q|k|v projection of this rank's Lp_rows
- * local tokens (A bf16 [Lp_rows, K], W bf16 [3C, K] = q|k|v weights stacked, bias f32 [3C]) on the SM-pair tcgen05 kernel whose
+ * local tokens (A bf16 [Lp_rows, K], W bf16 [3C, K] = q|k|v weights stacked, bias f32 [3C]) on the SM-pair wgmma kernel whose
  * EPILOGUE is the all-to-all: the columns of head h are stored straight into the receive buffer of the rank that owns h
  * (`peers[r]`, layout [P(src), Lp, q|k|v of heads/P] as for yb_sp_scatter_qkv), so the NVLink transfer rides under the GEMM's
  * main loop instead of a separate pass. WanRMSNorm spans all heads of a token, which no single receiver holds: the epilogue
@@ -321,10 +318,10 @@ int yb_vae_avgdown_add(void* main_, const void* x, int T, int H, int W, int in_c
 int yb_vae_patchify2_bf16(const void* video, void* out, long long ldo, int T, int H, int W, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
- * Self-test of the tcgen05 building blocks on one 128x128x128 tile (used by tests/, not by the product path).
+ * Self-test of the wgmma / TMA building blocks on one 128x128x128 tile (used by tests/, not by the product path).
  *   mode 0: A smem K-major, B smem K-major        D = A[128,128] * Bk[128(n),128(k)]^T
  *   mode 1: A smem K-major, B smem MN-major       D = A * Bmn[128(k),128(n)]
- *   mode 2: A in TMEM (bf16x2 packed), B MN-major D = A * Bmn
+ *   mode 2: A in registers (bf16x2 fragments), B MN-major D = A * Bmn
  * A, B bf16 [128,128] row-major; D f32 [128,128].
  * ------------------------------------------------------------------------------------------- */
 int yb_umma_probe(const void* A, const void* B, void* D, int mode, void* stream);  /* modes >= 3: A rows shifted by (mode - 2) */

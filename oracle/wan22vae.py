@@ -10,7 +10,7 @@ spatial padding), with two special cases that come from the first chunk:
     (channel groups [0:C] and [C:2C], :151-154);
   * `DupUp3D(first_chunk=True)` drops the first factor_t - 1 duplicated frames (:416-417).
 tests/golden/wan22vae_tiny.pt (tools/make_golden_vae22.py) is produced by the reference's own chunked code; the
-whole-sequence restatement below must reproduce it — that equivalence is what the B200 path relies on.
+whole-sequence restatement below must reproduce it — that equivalence is what the H100 path relies on.
 State-dict keys are the reference module tree's (`conv2.*`, `decoder.*`).
 """
 from __future__ import annotations

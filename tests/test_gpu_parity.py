@@ -55,7 +55,7 @@ def test_umma_probe(dev, mode):
                                        (2310, 3072, 512, 0), (2310, 3072, 512, 224), (1500, 704, 320, 160), (513, 96, 128, 32),
                                        (1029, 1184, 192, 192)])
 def test_gemm_pair_kernel_matches_1cta_kernel(dev, M, N, K, bn):
-    """SM-pair (`cta_group::2`) kernel, forced, against the 1-CTA kernel (bit-identical: same products, same fp32 accumulation
+    """SM-pair (2-CTA cluster) kernel, forced, against the 1-CTA kernel (bit-identical: same products, same fp32 accumulation
     order along K) and fp32 — ragged M / N tails, runtime N tiles (auto and forced), every fused epilogue."""
     from yume_b200 import ops
     g = torch.Generator(device="cpu").manual_seed(M + N + K)
@@ -242,11 +242,13 @@ def test_attention_kv_split_matches_unsplit(dev, Lq, Lk, heads, split):
 
 
 def test_attention_auto_tail_split_full_size_properties(dev):
-    """The 8-GPU Ulysses shape (3 heads, L = 18 480: 219 units on 148 SMs) takes the automatic tail split; compare the
-    whole output with the never-split launch."""
-    from yume_b200 import ops
+    """A full-length shape whose last wave is mostly idle (2 heads, L = 18 480: 146 units on the 132 SMs of an H100) takes the
+    automatic tail split; compare the whole output with the never-split launch."""
+    from yume_b200 import _lib, ops
     g = torch.Generator(device=dev).manual_seed(5)
-    L, heads = 18480, 3
+    L, heads = 18480, 2
+    sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    assert _lib.load().yb_attention_workspace_bytes(L, L, heads, sms, 0) > 0   # the automatic plan splits this launch
     q, k, v = (torch.randn(L, heads * 128, generator=g, device=dev).bfloat16() for _ in range(3))
     a = ops.attention(q, k, v, torch.empty_like(q), heads, split=1)
     b = ops.attention(q, k, v, torch.full_like(q, 7.0), heads, split=0)

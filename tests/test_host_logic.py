@@ -249,21 +249,22 @@ def test_attention_tail_split_plan():
     from yume_b200 import _lib
     lib = _lib.load()
 
-    def plan(Lq, Lk, heads, sms=148, flags=0):
+    def plan(Lq, Lk, heads, sms=132, flags=0):
         out = (C.c_int * 4)()
         assert lib.yb_attention_plan(Lq, Lk, heads, sms, flags, out) == 0
         return tuple(out)
 
-    L = 18480
-    assert plan(L, L, 3) == (148, 71, 2, 74)              # 8 GPUs: 219 units = 1.48 waves -> 71 tail units in two KV halves
-    for heads in (24, 12, 6):                             # 1 / 2 / 4 GPUs: last wave more than half full, no split
+    L = 18480                                             # 73 units of 256 query rows per head, on the 132 SMs of an H100
+    assert plan(L, L, 24) == (1716, 36, 3, 50)            # 1 GPU: 1752 units = 13.27 waves -> 36 tail units in three KV segments
+    assert plan(L, L, 6) == (396, 42, 3, 50)              # 4 GPUs: 438 units = 3.32 waves -> 42 tail units in three KV segments
+    for heads in (12, 3):                                 # 2 / 8 GPUs: last wave more than half full, no split
         full, tail, ns, per = plan(L, L, heads)
         assert (tail, ns) == (0, 1) and full == heads * 73 and per == 145
-    assert plan(L, L, 3, flags=2)[1] == 0                 # YB_ATT_ACCUMULATE launches never split
-    assert plan(L, L, 3, flags=1 << 4)[1] == 0            # split policy 1 = never
+    assert plan(L, L, 6, flags=2)[1] == 0                 # YB_ATT_ACCUMULATE launches never split
+    assert plan(L, L, 6, flags=1 << 4)[1] == 0            # split policy 1 = never
     assert plan(300, 512, 2, flags=2 << 4) == (0, 4, 2, 2)    # forced: every unit, 4 key tiles -> 2 + 2
     assert plan(300, 256, 2, flags=2 << 4)[1] == 0            # too few key tiles to split
-    assert lib.yb_attention_plan(0, 1, 1, 148, 0, (C.c_int * 4)()) != 0
+    assert lib.yb_attention_plan(0, 1, 1, 132, 0, (C.c_int * 4)()) != 0
     import itertools
     for Lq, Lk, heads, sms, force in itertools.product((1, 255, 257, 5000, 18480, 40000), (1, 129, 2049, 18480, 33000),
                                                        (1, 3, 5, 24), (1, 132, 148), (0, 2, 3, 4)):
@@ -304,24 +305,24 @@ def test_conv_tile_plan():
 
 
 @pytest.mark.parametrize("tree,cfg_name", [("wan23", "CFG_5B_TINY"), ("wan", "CFG_14B_TINY")])
-def test_install_on_the_reference_wanmodel_repacks_identically(tree, cfg_name):
-    """Drop-in boundary (SURVEY.md §8b): `install()` on a live REFERENCE `WanModel` — loaded from /root/reference with the
-    recipe of tools/make_golden.py — must re-bind `forward` and build, from the module's own parameters
-    (`WanDiT.from_module`), exactly the packed tensors the state-dict path builds. Runs where the reference tree exists (the
-    authoring container); skipped on the GPU box."""
-    import sys
-    ref_root = Path("/root/reference")
-    if not (ref_root / tree / "modules" / "model.py").exists():
-        pytest.skip("reference tree not present")
-    sys.path.insert(0, str(ROOT / "tools"))
-    import make_golden
+def test_install_on_the_reference_wanmodel_repacks_identically(golden_dir, tree, cfg_name):
+    """Drop-in boundary (SURVEY.md §8b): `install()` on a live `WanModel` — the repo's mirror of the reference class, whose state-dict
+    keys and shapes must equal those recorded from the reference's own `WanModel` (tests/golden/install_hooks.pt,
+    tools/make_golden_install.py) — must re-bind `forward` and build, from the module's own parameters (`WanDiT.from_module`), exactly
+    the packed tensors the state-dict path builds."""
     from yume_b200 import model as ybm
     cfg = getattr(synth, cfg_name)
     sd = synth.make_state_dict(cfg, 4321)
-    ref_model = make_golden.build_reference_model(make_golden.load_reference(tree), cfg, sd)
-    assert type(ref_model).__module__.startswith(tree)                 # really the reference's class
+    kw = dict(text_len=cfg["text_len"], in_dim=cfg["in_dim"], dim=cfg["dim"], ffn_dim=cfg["ffn_dim"], freq_dim=cfg["freq_dim"],
+              text_dim=cfg["text_dim"], out_dim=cfg["out_dim"], num_heads=cfg["num_heads"], num_layers=cfg["num_layers"])
+    ref_model = (ybm.WanModel5B(model_type="ti2v", **kw) if cfg["variant"] == "5b"
+                 else ybm.WanModel14B(model_type="i2v", clip_dim=cfg["clip_dim"], **kw))
+    want_keys = torch.load(golden_dir / "install_hooks.pt")["wanmodel"][tree]
+    assert {k: tuple(v.shape) for k, v in ref_model.state_dict().items()} == want_keys   # the reference class's state-dict interface
+    ref_model.load_state_dict(sd, strict=True)
+    ref_model.eval()
     ref_forward = ref_model.forward
-    ybm.install(ref_model, device="cpu")                               # repack only: no kernel runs at install time
+    ybm.install(ref_model, device="cpu")                               # repack only, from the live parameters: no kernel runs
     assert ref_model.forward is not ref_forward and ref_model.forward.__func__ in (ybm.forward_5b, ybm.forward_14b)
     eng = ref_model._yb_engine
     kw = synth.oracle_kwargs(cfg)
@@ -390,50 +391,52 @@ def test_ctypes_structs_match_the_c_header(tmp_path):
 
 
 def test_gemm_plan_kernel_choice():
-    """Host-side kernel / tile choice of yb_gemm_bf16 (yb_gemm_plan): the SM-pair kernel with 256-wide tiles for the token GEMMs,
-    the 1-CTA kernel for the small context / embedding projections."""
+    """Host-side kernel / tile choice of yb_gemm_bf16 (yb_gemm_plan): the 1-CTA kernel for every shape (the SM-pair form runs at
+    half its rate on the H100), 256-wide tiles when N allows, 128-wide for narrow outputs."""
     import ctypes as C
     lib = yume_b200.load()
     out = (C.c_int * 4)()
 
     def plan(M, N):
-        assert lib.yb_gemm_plan(M, N, 148, out) == 0
+        assert lib.yb_gemm_plan(M, N, 132, out) == 0
         return tuple(out)
-    assert plan(18480, 3072) == (1, 256, 73, 12)
-    assert plan(18480, 14336) == (1, 256, 73, 56)
-    assert plan(2310, 9216) == (1, 256, 10, 36)
-    assert plan(1024, 128) == (1, 128, 4, 1)
-    assert plan(512, 3072) == (0, 256, 4, 12)            # context rows: 1-CTA kernel
+    assert plan(18480, 3072) == (0, 256, 145, 12)
+    assert plan(18480, 14336) == (0, 256, 145, 56)
+    assert plan(2310, 9216) == (0, 256, 19, 36)
+    assert plan(1024, 128) == (0, 128, 8, 1)
+    assert plan(512, 3072) == (0, 256, 4, 12)            # context rows
     assert plan(257, 96) == (0, 128, 3, 1)
-    assert lib.yb_gemm_plan(0, 128, 148, out) != 0
+    assert lib.yb_gemm_plan(0, 128, 132, out) != 0
 
 
 def test_gemm_tail_split_k_plan():
-    """The split-K chooser of the SM-pair gate+residual GEMM (host arithmetic, no GPU): splits the per-rank shapes of 4- / 8-GPU
-    Ulysses whose last wave is mostly idle, leaves full last waves and short-K launches alone, and every segment owns K blocks."""
+    """The split-K chooser of the SM-pair gate+residual GEMM (host arithmetic, no GPU) on the 66 SM pairs of an H100: splits the
+    launches whose last wave is mostly idle, leaves the ones whose tail needs several sub-waves alone, and every segment owns K
+    blocks. The automatic choices are the ones measured fastest on an H100 (gemm.cu, gemm_splitk_plan)."""
     import ctypes as C
     lib = yume_b200.load()
     out = (C.c_int * 3)()
 
-    def plan(tiles, num_kb, clusters=74, force=0):
+    def plan(tiles, num_kb, clusters=66, force=0):
         assert lib.yb_gemm_splitk_plan(tiles, num_kb, clusters, force, out) == 0
         return tuple(out)
 
-    assert plan(120, 224)[1] == 1                 # 8 GPUs, FFN-down: 46 tail tiles need two sub-waves; measured gain 1 %: left alone
-    assert plan(120, 224, force=3) == (74, 3, 75)
-    assert plan(120, 48)[1] == 1                  # 8 GPUs, o-projection: the combine launch costs more than the idle tail
-    full, ns, per = plan(228, 224)                # 4 GPUs, FFN-down: 6 tail tiles spread over the 74 pairs
-    assert full == 222 and ns >= 6 and 6 * ns <= 74 and (ns - 1) * per < 224 <= ns * per
-    assert plan(876, 224)[1] == 1 and plan(444, 224)[1] == 1     # 1 / 2 GPUs: last wave (nearly) full
-    assert plan(74, 224) == (74, 1, 224) and plan(50, 224)[1] == 1
-    assert plan(100, 224, force=2) == (74, 2, 112) and plan(100, 224, force=1)[1] == 1
+    assert plan(120, 224)[1] == 1                 # M 2310 x N 3072, K 14336: 54 tail tiles need two sub-waves; measured slower: left alone
+    assert plan(120, 224, force=3) == (66, 3, 75)
+    assert plan(120, 48)[1] == 1                  # M 2310, K 3072: measured slower split: left alone
+    assert plan(228, 224) == (198, 2, 112)        # M 4620, K 14336: 30 tail tiles in two segments (measured best)
+    assert plan(228, 48) == (198, 2, 24)          # M 4620, K 3072: the same (measured best)
+    assert plan(72, 48) == (66, 6, 8)             # M 1500, K 3072: 6 tail tiles spread over the pairs (measured best)
+    assert plan(132, 224)[1] == 1                 # full last wave
+    assert plan(66, 224) == (66, 1, 224) and plan(50, 224)[1] == 1
+    assert plan(100, 224, force=2) == (66, 2, 112) and plan(100, 224, force=1)[1] == 1
     assert plan(5, 8, force=2) == (0, 2, 4) and plan(5, 3, force=2)[1] == 1
     for tiles in range(1, 400, 7):
         for num_kb in (8, 48, 80, 224):
             full, ns, per = plan(tiles, num_kb)
             assert 0 <= full <= tiles and 1 <= ns <= 12
             if ns > 1:
-                assert full % 74 == 0 and (ns - 1) * per < num_kb <= ns * per and per >= 8
+                assert full % 66 == 0 and (ns - 1) * per < num_kb <= ns * per and per >= 8
 
 
 def test_graft_entry_build_runs():

@@ -1,9 +1,10 @@
-"""Drop-in hooks of the Wan VAEs on the REFERENCE's own classes, on CPU: build `WanVAE_` from /root/reference (2.2 and 2.1 trees) with
-seeded weights, wrap it the way `Wan2_2_VAE` / `WanVAE` hold it (`.model`, `.scale` / `.mean`, `.std`; their constructors want a
-checkpoint file), run the reference's own chunked encode / decode, then `install_*` on the wrapper and call `encode(list)` /
-`decode(list)` — list in / list out, outputs within the bf16 budget of the reference's fp32 result. The engines run over the torch
-stand-in for the C ABI (tests/helpers/torch_ops.py). Authoring container only (skipped where /root/reference is absent)."""
-import importlib.util
+"""Drop-in hooks of the VAEs against the REFERENCE's own objects, on CPU. tools/make_golden_install.py built the reference's `WanVAE_`
+(2.2 and 2.1 trees) and `AutoencoderKLCausal3D` with seeded weights and stored, in tests/golden/install_hooks.pt, what the hooks read
+from them (the attributes, the state-dict keys and shapes, `config` and the tiling switches) and what their own encode / decode
+returned. Here the hooks are installed on stand-ins that expose exactly that recorded interface, and `encode(list)` / `decode(list)`
+/ `decode(z, return_dict=...)` must keep the reference's calling convention and land within the bf16 budget of its fp32 result. The
+engines run over the torch stand-in for the C ABI (tests/helpers/torch_ops.py)."""
+import sys
 import types
 from pathlib import Path
 
@@ -11,10 +12,10 @@ import pytest
 import torch
 
 from helpers import torch_ops
-from oracle import wan21vae, wan21vae_enc, wan22vae, wan22vae_enc
 from yume_b200 import vae21, vae22, vae_enc
 
-REF = Path("/root/reference")
+sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tools"))
+import make_golden_install as recipe  # noqa: E402
 
 
 @pytest.fixture()
@@ -23,97 +24,71 @@ def cpu_ops(monkeypatch):
         monkeypatch.setattr(mod, "ops", torch_ops)
 
 
-def _load(path, name):
-    if not path.exists():
-        pytest.skip("reference tree not present")
-    spec = importlib.util.spec_from_file_location(name, str(path))
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    return mod
+@pytest.fixture(scope="module")
+def golden(golden_dir):
+    return torch.load(golden_dir / "install_hooks.pt")
 
 
 def _rel(a, b):
     return float((a.float() - b.float()).norm() / b.float().norm())
 
 
+def _wan_model(g, sd):
+    """stand-in for the reference `WanVAE_`: its recorded attributes and a state dict with the recorded keys and shapes"""
+    assert {k: tuple(v.shape) for k, v in sd.items()} == g["keys"]
+    return types.SimpleNamespace(state_dict=lambda: dict(sd), **g["attrs"])
+
+
 @torch.no_grad()
-def test_wan22_wrapper_hooks_are_drop_ins(cpu_ops):
-    ref = _load(REF / "wan23" / "modules" / "vae2_2.py", "ref_vae2_2_install")
-    cfg = dict(dim=32, z_dim=16, dim_mult=(1, 2, 4, 4), num_res_blocks=2, temperal_downsample=(False, True, True))
-    sd = dict(wan22vae_enc.make_state_dict(11, **cfg))
-    sd.update(wan22vae.make_state_dict(12, dec_dim=32, z_dim=16, dim_mult=(1, 2, 4, 4), num_res_blocks=2, temperal_upsample=(True, True, False)))
-    model = ref.WanVAE_(dim=32, dec_dim=32, z_dim=16, dim_mult=[1, 2, 4, 4], num_res_blocks=2, attn_scales=[],
-                        temperal_downsample=[False, True, True]).eval()
-    model.load_state_dict(sd, strict=True)
-    g = torch.Generator().manual_seed(3)
-    mean, std = 0.3 * torch.randn(16, generator=g), 0.5 + torch.rand(16, generator=g)
-    wrapper = types.SimpleNamespace(model=model, scale=[mean, 1.0 / std], dtype=torch.float)
-    video = torch.randn(3, 5, 32, 64, generator=g).clamp_(-1, 1)
-    z = torch.randn(16, 2, 2, 4, generator=g)
-    want_mu = model.encode(video.unsqueeze(0), wrapper.scale).float().squeeze(0)
-    want_x = model.decode(z.unsqueeze(0), wrapper.scale).float().clamp_(-1, 1).squeeze(0)
+def test_wan22_wrapper_hooks_are_drop_ins(cpu_ops, golden):
+    g = golden["wan22"]
+    mean, std, video, z = recipe.wan_vae_inputs("wan22")
+    wrapper = types.SimpleNamespace(model=_wan_model(g, recipe.wan22_state_dict()), scale=[mean, 1.0 / std], dtype=torch.float)
     vae_enc.install_wan22_vae_encoder(wrapper, device="cpu")
     vae22.install_wan22_vae(wrapper, device="cpu")
     got_mu, got_x = wrapper.encode([video]), wrapper.decode([z])
     assert isinstance(got_mu, list) and isinstance(got_x, list) and len(got_mu) == len(got_x) == 1
-    assert got_mu[0].shape == want_mu.shape and _rel(got_mu[0], want_mu) < 3e-2
-    assert got_x[0].shape == want_x.shape and _rel(got_x[0], want_x) < 3e-2
+    assert got_mu[0].shape == g["mu"].shape and _rel(got_mu[0], g["mu"]) < 3e-2
+    assert got_x[0].shape == g["x"].shape and _rel(got_x[0], g["x"]) < 3e-2
     assert wrapper.encode(video) is None and wrapper.decode(z) is None          # the reference logs a TypeError and returns None
 
 
 @torch.no_grad()
-def test_wan21_wrapper_hooks_are_drop_ins(cpu_ops):
-    ref = _load(REF / "wan" / "modules" / "vae.py", "ref_vae_install")
-    cfg = dict(dim=32, z_dim=16, dim_mult=(1, 2, 4, 4), num_res_blocks=2)
-    sd = dict(wan21vae_enc.make_state_dict(21, temperal_downsample=(False, True, True), **cfg))
-    sd.update(wan21vae.make_state_dict(22, temperal_upsample=(True, True, False), **cfg))
-    model = ref.WanVAE_(dim=32, z_dim=16, dim_mult=[1, 2, 4, 4], num_res_blocks=2, attn_scales=[], temperal_downsample=[False, True, True]).eval()
-    model.load_state_dict(sd, strict=True)
-    g = torch.Generator().manual_seed(4)
-    mean, std = 0.3 * torch.randn(16, generator=g), 0.5 + torch.rand(16, generator=g)
-    wrapper = types.SimpleNamespace(model=model, mean=mean, std=std, scale=[mean, 1.0 / std], dtype=torch.float)
-    video = torch.randn(3, 5, 16, 32, generator=g).clamp_(-1, 1)
-    z = torch.randn(16, 2, 2, 4, generator=g)
-    want_mu = model.encode(video.unsqueeze(0), wrapper.scale).float().squeeze(0)
-    want_x = model.decode(z.unsqueeze(0), wrapper.scale).float().clamp_(-1, 1).squeeze(0)
+def test_wan21_wrapper_hooks_are_drop_ins(cpu_ops, golden):
+    g = golden["wan21"]
+    mean, std, video, z = recipe.wan_vae_inputs("wan21")
+    wrapper = types.SimpleNamespace(model=_wan_model(g, recipe.wan21_state_dict()), mean=mean, std=std, scale=[mean, 1.0 / std],
+                                    dtype=torch.float)
     vae_enc.install_wan21_vae_encoder(wrapper, device="cpu")
     vae21.install_wan21_vae(wrapper, device="cpu")
     got_mu, got_x = wrapper.encode([video]), wrapper.decode([z])
-    assert got_mu[0].shape == want_mu.shape and _rel(got_mu[0], want_mu) < 3e-2
-    assert got_x[0].shape == want_x.shape and _rel(got_x[0], want_x) < 3e-2
+    assert got_mu[0].shape == g["mu"].shape and _rel(got_mu[0], g["mu"]) < 3e-2
+    assert got_x[0].shape == g["x"].shape and _rel(got_x[0], g["x"]) < 3e-2
 
 
 @torch.no_grad()
-def test_hyvideo_install_vae_is_a_drop_in(monkeypatch):
-    """`install_vae` on the reference's own `AutoencoderKLCausal3D` (hyvideo/vae/autoencoder_kl_causal_3d.py, loaded with the diffusers
-    stubs of tools/make_golden_vae.py): the module's own tiled decode, then the re-bound `decode(z, return_dict=...)` — same return
-    convention, `enable_tiling()` honoured, output within the bf16 budget."""
-    import sys
-    if not (REF / "hyvideo" / "vae" / "autoencoder_kl_causal_3d.py").exists():
-        pytest.skip("reference tree not present")
-    root = Path(__file__).resolve().parents[1]
-    sys.path.insert(0, str(root / "tools"))
-    import make_golden_vae
+def test_hyvideo_install_vae_is_a_drop_in(monkeypatch, golden):
+    """`install_vae` on a stand-in with the reference `AutoencoderKLCausal3D`'s config, tiling switches and decoder state dict: the
+    re-bound `decode(z, return_dict=...)` keeps the return convention, follows the module's tiling switches, and matches the reference's
+    tiled decode (a fixed seeded sample of it) and its untiled decode of a small latent."""
     from oracle import hyvae
     from yume_b200 import vae as ybvae
     monkeypatch.setattr(ybvae, "ops", torch_ops)
-    ak = make_golden_vae.load_reference_vae()
-    cfg = make_golden_vae.TINY
-    sd = hyvae.make_state_dict(99, **cfg)
-    ref = ak.AutoencoderKLCausal3D(in_channels=3, out_channels=3, down_block_types=("DownEncoderBlockCausal3D",) * 4,
-                                   up_block_types=("UpDecoderBlockCausal3D",) * 4, block_out_channels=cfg["block_out_channels"],
-                                   layers_per_block=2, act_fn="silu", latent_channels=16, norm_num_groups=32, sample_size=64,
-                                   sample_tsize=16, time_compression_ratio=4, spatial_compression_ratio=8, mid_block_add_attention=True)
-    ref.load_state_dict(sd, strict=False)
-    ref.eval()
-    ref.enable_tiling()
-    z = torch.randn(1, 16, 6, 10, 12, generator=torch.Generator().manual_seed(5))
-    want = ref.decode(z, return_dict=False)[0]
+    g = golden["hyvae"]
+    import make_golden_vae
+    sd = hyvae.make_state_dict(99, **make_golden_vae.TINY)
+    sd = {k: v for k, v in sd.items() if k in g["keys"]}
+    assert {k: tuple(v.shape) for k, v in sd.items()} == g["keys"]
+    ref = types.SimpleNamespace(config=dict(g["config"]), state_dict=lambda: dict(sd))
+    ref.use_spatial_tiling, ref.use_temporal_tiling = g["tiling_on"]                # what enable_tiling() leaves
+    z, small = recipe.hy_latents()
     ybvae.install_vae(ref, device="cpu")
     got = ref.decode(z, return_dict=False)
-    assert isinstance(got, tuple) and got[0].shape == want.shape and _rel(got[0], want) < 3e-2
+    assert isinstance(got, tuple) and tuple(got[0].shape) == g["tiled_shape"]
+    idx = recipe.hy_sample_index(got[0].numel())
+    assert _rel(got[0].reshape(-1)[idx], g["tiled_sample"]) < 3e-2
     out = ref.decode(z)
-    assert _rel(out.sample, want) < 3e-2
-    ref.disable_tiling()                                          # the hook follows the module's own switches
-    small = torch.randn(1, 16, 2, 4, 6, generator=torch.Generator().manual_seed(6))
-    assert ref.decode(small, return_dict=False)[0].shape == (1, 3, 5, 32, 48)
+    assert _rel(out.sample.reshape(-1)[idx], g["tiled_sample"]) < 3e-2
+    ref.use_spatial_tiling, ref.use_temporal_tiling = g["tiling_off"]               # what disable_tiling() leaves
+    small_out = ref.decode(small, return_dict=False)[0]
+    assert small_out.shape == g["untiled_small"].shape == (1, 3, 5, 32, 48) and _rel(small_out, g["untiled_small"]) < 3e-2

@@ -39,7 +39,7 @@ def sec_probe():
         alt = a.float() @ (b.float() if mode == 0 else b.float().t())
         print(f"probe mode {mode}: rel/max vs expected {rel(d, ref)}  vs transposed-B {rel(d, alt)}  finite={torch.isfinite(d).all().item()}")
         if mode == 2:
-            # hypothesis check: swapped bf16 halves in the TMEM A operand
+            # hypothesis check: swapped bf16 halves in the register A operand
             a_sw = a.view(128, 64, 2).flip(-1).reshape(128, 128)
             print("   vs half-swapped A:", rel(d, a_sw.float() @ b.float()))
 
@@ -340,43 +340,7 @@ def sec_convpair():
         print(line + f"  equal={torch.equal(outs[0], outs[2])} fused_rel={rel(outs[1], outs[0])[0]:.1e}", flush=True)
 
 
-def sec_atttrace():
-    from yume_b200 import _lib
-    heads, L = 24, 18480
-    qkv = torch.randn(L, 3 * heads * 128, device=dev).bfloat16()
-    q = qkv[:, : heads * 128]; k = qkv[:, heads * 128: 2 * heads * 128]; v = qkv[:, 2 * heads * 128:]
-    out = torch.empty(L, heads * 128, device=dev, dtype=torch.bfloat16)
-    tr = torch.zeros(32 * 32, device=dev, dtype=torch.int64)
-    lib = _lib.load()
-    _trace_one(lib, q, k, v, out, tr, L, heads, 0)
-
-
-def _trace_one(lib, q, k, v, out, tr, L, heads, flags=0):
-    for _ in range(3):
-        rc = lib.yb_attention_ex(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0), out.data_ptr(),
-                                 out.stride(0), L, L, heads, 1.0 / math.sqrt(128.0), flags, None, 0, tr.data_ptr(), torch.cuda.current_stream().cuda_stream)
-        assert rc == 0
-    torch.cuda.synchronize()
-    t = tr.view(32, 32).cpu()
-    base = t[0, 1].item()
-    names = ["sm_wait_S", "ldS", "max", "exp_half0+st", "exp_half1+st"]
-    for X in (0, 1):
-        d = t[:, X * 8: X * 8 + 6]
-        seg = (d[:, 1:] - d[:, :-1]).float()
-        print(f"softmax tile {X}: mean cycles per phase:", {n: round(seg[:, i].mean().item()) for i, n in enumerate(names)},
-              " iteration period:", round((d[1:, 1] - d[:-1, 1]).float().mean().item()))
-    for X in (0, 1):
-        d = t[:, 16 + X * 4: 16 + X * 4 + 3]
-        print(f"mma tile {X}: wait_P {round((d[:,1]-d[:,0]).float().mean().item())}  issue {round((d[:,2]-d[:,1]).float().mean().item())}")
-    # handoff latencies: P arrive (softmax) -> MMA sees P; MMA issue end -> softmax sees S of next tile
-    for X in (0, 1):
-        arrive = t[:, X * 8 + 5]; p_seen = t[:, 16 + X * 4 + 1]; issued = t[:, 16 + X * 4 + 2]
-        s_seen_next = t[1:, X * 8 + 1]
-        print(f"tile {X}: arrive->P seen {round((p_seen - arrive).float().mean().item())}; issue end -> S(j+1) seen {round((s_seen_next - issued[:-1]).float().mean().item())}")
-    print("raw rows 0..2:", (t[:3] - base).tolist())
-
-
-SECTIONS = {"attmodes": sec_attmodes, "gemmpair": sec_gemmpair, "gemmsplit": sec_gemmsplit, "convpair": sec_convpair, "attsplit": sec_attsplit, "atttrace": sec_atttrace, "atttune": sec_atttune, "probe": sec_probe, "gemm": sec_gemm, "attention": sec_attention, "elementwise": sec_elementwise}
+SECTIONS = {"attmodes": sec_attmodes, "gemmpair": sec_gemmpair, "gemmsplit": sec_gemmsplit, "convpair": sec_convpair, "attsplit": sec_attsplit, "atttune": sec_atttune, "probe": sec_probe, "gemm": sec_gemm, "attention": sec_attention, "elementwise": sec_elementwise}
 if __name__ == "__main__":
     names = sys.argv[1:] or [n for n in SECTIONS if n not in ("gemmpair", "attmodes", "convpair", "gemmsplit")]   # experimental sections only on request
     print(torch.cuda.get_device_name(0))

@@ -1,4 +1,4 @@
-"""yume_b200 — B200-native (sm_100a) implementation of YUME's denoise hot path behind the reference's own seams.
+"""yume_b200 — H100-native (sm_90a) implementation of YUME's denoise hot path behind the reference's own seams.
 
 Public surface:
   yume_b200.install(model)          re-bind `WanModel.forward` of a live reference model (yume_b200.model)

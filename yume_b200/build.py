@@ -1,4 +1,4 @@
-"""Build libyume_b200.so (sm_100a only) in-tree with nvcc.
+"""Build libyume_b200.so (sm_90a only) in-tree with nvcc.
 
 The library is plain C ABI (include/yume_b200.h); there is no torch / pybind dependency in it, so it is built
 with a direct nvcc invocation rather than torch.utils.cpp_extension. nvcc cross-compiles without a GPU.
@@ -19,7 +19,7 @@ SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "vae_elementwise.cu", "p
 HEADERS = ["yb_ptx.cuh", "yb_host.h", "../../include/yume_b200.h"]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
             raise RuntimeError(f"nvcc failed on {src}")
         objs.append(str(obj))
     tmp = LIB.with_suffix(".so.tmp")          # link beside the target, then rename: a reader never sees a half-written library
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", str(tmp), *objs]
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", str(tmp), *objs]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         sys.stderr.write(r.stdout)

@@ -1,6 +1,5 @@
-// attention.cu — FlashAttention-style forward for sm_100a: TMA-staged Q/K/V tiles, tcgen05.mma with fp32
-// accumulators in TMEM, online softmax in registers (one thread per query row), P fed back to the tensor
-// core from TMEM (or shared memory, variant 1).
+// attention.cu — FlashAttention-style forward for sm_90a (H100): TMA-staged Q/K/V tiles, wgmma with fp32 accumulators in
+// registers, online softmax in registers, P fed back to the tensor core from registers (or shared memory, variant 1).
 //
 // Replaces flash_attention(q, k, v, k_lens) as used by WanSelfAttention / WanCrossAttention
 // (reference: wan23/modules/attention.py:24-130 -> flash_attn_varlen_func; call sites
@@ -8,19 +7,14 @@
 // Contract kept: non-causal, softmax scale 1/sqrt(D), keys >= k_len dropped, bf16 inputs, fp32 accumulate,
 // output in [L, heads, D] layout (so the o-projection GEMM reads it directly). Batch is 1 on every Yume path.
 //
-// CTA = 2 query tiles of 128 rows (ping-pong), one head. 384 threads:
-//   warp 0        TMA producer (Q once; K_j / V_j through an smem ring)
-//   warp 1        MMA issuer (single thread): S_X = Q_X K_j^T  and  O_X += P_X V_j
-//   warps 4-7     softmax for query tile 0: thread t owns row t (TMEM lane t)
-//   warps 8-11    softmax for query tile 1
-// TMEM columns: [0,128) S_0 / P_0, [128,256) S_1 / P_1, [256,384) O_0, [384,512) O_1.
-// Issue order per KV tile j: PV_0(j), S_0(j+1), PV_1(j), S_1(j+1) — while the tensor core works on tile X
-// the softmax warps of tile 1-X run. O is rescaled lazily (only when a row max grows by > 2^8).
+// CTA = one work unit of 256 query rows of one head, run as two 128-row query tiles one after the other. 384 threads:
+//   warpgroup 0     TMA producer (one thread): Q tile, then K_j / V_j through an smem ring
+//   warpgroups 1-2  query rows [64*(wg-1), +64) of the current tile: S = Q K_j^T (wgmma, both operands in smem), masking and
+//                   online softmax on the accumulator fragment, O += P V_j with P as the register A operand
 //
-// Tail split: a launch is U = heads x ceil(Lq/256) equal work units on 148 SMs. When the last wave is at most half
-// full (8-GPU Ulysses: 3 heads x 73 = 219 units = 1.48 waves) its T units are each cut into ns = floor(148 / T) KV
-// segments that run as separate CTAs and leave (unnormalised O, row max, row sum) in a workspace; a small combine
-// kernel merges the segments and performs the normal epilogue (bf16 store / Ulysses peer scatter). 2 waves -> 1.5.
+// Tail split: a launch is U = heads x ceil(Lq/256) equal work units. When the last wave is at most half full its T units are each
+// cut into ns KV segments that run as separate CTAs and leave (unnormalised O, row max, row sum) in a workspace; a small combine
+// kernel merges the segments and performs the normal epilogue (bf16 store / Ulysses peer scatter).
 #include "yb_host.h"
 #include "yb_ptx.cuh"
 
@@ -39,7 +33,6 @@ struct AttParams {
   // [P(src), Lp, heads_local*128] receive buffer over NVLink (peer pointers) — the all-to-all is the epilogue itself.
   __nv_bfloat16* out_peers[8];
   int sp_world, sp_rank, sp_Lp;
-  long long* trace;  // optional clock64 trace of CTA (1,0), KV tiles 16..47 (tests/tools only; null in production)
   float scale_log2;  // softmax scale * log2(e)
   // work decomposition: unit u = head * nq + q_block. CTAs [0, full_units) run whole units; CTA full_units + r runs KV
   // segment r % ns of unit full_units + r / ns and writes a partial result to the workspace
@@ -48,407 +41,234 @@ struct AttParams {
   float* ws_ml;      // [tail CTAs, 256, 2]   (row max in the log2 domain, row sum)
 };
 
-// Epilogue shared by the attention kernels: thread = query row (TMEM lane), tO = its O accumulator. A KV segment of a tail unit
-// leaves (unnormalised O, m, l) in the workspace for attention_combine_kernel; a whole unit stores O / l as bf16 into
-// out[Lq, heads*128] (accumulating, or into the owner rank's receive buffer under Ulysses).
-__device__ __forceinline__ void attention_epilogue(const AttParams& p, uint32_t tO, float m_used, float l, int X, int row_in_tile,
-                                                   int unit) {
-  if (static_cast<int>(blockIdx.x) >= p.full_units) {
-    const long long prow = static_cast<long long>(blockIdx.x - p.full_units) * 256 + X * 128 + row_in_tile;
-    float* wo = p.ws_o + prow * 128;
-    *reinterpret_cast<float2*>(p.ws_ml + prow * 2) = make_float2(m_used, l);
-#pragma unroll 1
-    for (int c = 0; c < 4; ++c) {
-      uint32_t o[32];
-      tmem_ld32(tO + c * 32, o);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 8; ++i)
-        *reinterpret_cast<uint4*>(wo + c * 32 + 4 * i) = make_uint4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-    }
-    return;
-  }
-  const int head = unit / p.nq;
-  const int q0 = (unit - head * p.nq) * 256;
-  const float inv = 1.0f / l;
-  const int q_row = q0 + X * 128 + row_in_tile;
-  __nv_bfloat16* orow = p.out + static_cast<long long>(q_row) * p.ldo + head * 128;
-  if (p.sp_world > 1) {
-    const int owner = q_row / p.sp_Lp;
-    const int t = q_row - owner * p.sp_Lp;
-    if (owner < p.sp_world)
-      orow = p.out_peers[owner] + (static_cast<long long>(p.sp_rank) * p.sp_Lp + t) * p.ldo + head * 128;
-  }
-#pragma unroll 1
-  for (int c = 0; c < 4; ++c) {
-    uint32_t o[32];
-    tmem_ld32(tO + c * 32, o);
-    tmem_ld_wait();
-    if (q_row < p.Lq) {
-      uint4* o4 = reinterpret_cast<uint4*>(orow + c * 32);
-      if (p.accumulate) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const uint4 prev = o4[i];
-          const __nv_bfloat162* ph = reinterpret_cast<const __nv_bfloat162*>(&prev);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const float2 f = __bfloat1622float2(ph[k]);
-            o[8 * i + 2 * k] = __float_as_uint(__uint_as_float(o[8 * i + 2 * k]) + f.x * l);
-            o[8 * i + 2 * k + 1] = __float_as_uint(__uint_as_float(o[8 * i + 2 * k + 1]) + f.y * l);
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        uint4 w;
-        w.x = pack_bf16x2(__uint_as_float(o[8 * i + 0]) * inv, __uint_as_float(o[8 * i + 1]) * inv);
-        w.y = pack_bf16x2(__uint_as_float(o[8 * i + 2]) * inv, __uint_as_float(o[8 * i + 3]) * inv);
-        w.z = pack_bf16x2(__uint_as_float(o[8 * i + 4]) * inv, __uint_as_float(o[8 * i + 5]) * inv);
-        w.w = pack_bf16x2(__uint_as_float(o[8 * i + 6]) * inv, __uint_as_float(o[8 * i + 7]) * inv);
-        o4[i] = w;
-      }
-    }
-  }
-}
-
-template <bool P_TMEM>
+template <bool P_SMEM>
 struct AttCfg {
-  static constexpr int NS = P_TMEM ? 5 : 3;  // KV ring slots
+  static constexpr int NS = P_SMEM ? 4 : 5;  // KV ring slots
   static constexpr int Q_OFF = 0;
-  static constexpr int P_OFF = 2 * ATT_TILE_BYTES;
-  static constexpr int KV_OFF = P_TMEM ? 2 * ATT_TILE_BYTES : 4 * ATT_TILE_BYTES;
+  static constexpr int P_OFF = ATT_TILE_BYTES;   // P_SMEM: 64 x 128 bf16 per consumer warpgroup (2 slabs of 8 KB)
+  static constexpr int KV_OFF = P_SMEM ? 2 * ATT_TILE_BYTES : ATT_TILE_BYTES;
   static constexpr int BAR_OFF = KV_OFF + NS * ATT_TILE_BYTES;
-  static constexpr int SMEM_BYTES = BAR_OFF + 1024 + 256;
+  static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;
+  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 };
 
-// Where the time goes (profiles/r02_ncu_block.md, r02_instr_rate.md): per 128-key step a CTA spends ~3000 cycles for 2048 cycles of tensor
-// work and 2048 cycles of MUFU work; both pipes are ~67 % busy. Each query tile's chain softmax (~1720) -> P.V + next S (~1150) ->
-// hand-off (~100) is serial, the two tiles run it in ping-pong. The exponential phase of the one softmax warp per scheduler runs at
-// 10.9 cycles per MUFU.EX2 (21.9 per pair of scores): the unit alone issues every 8.0 cycles, every 8.5 - 9.0 while the tensor core of
-// the SM is busy, and this instruction mix on one warp takes 20.0 per pair under tensor load (ptxas schedules it at 8.1 per MUFU, the
-// rest are scoreboard waits of an in-order warp) — the phase is within 10 % of what its instruction stream can do.
-// Round 2 measured eleven alternatives against this kernel and kept none (profiles/r02_attention_schedules.md): Q in TMEM with 64-key tiles, deferred max, packed bf16x2 exponentials, pipelined softmax, ALU-pipe packing, FMA-pipe
-// polynomial exponentials, a lookahead schedule with double-buffered S, scalar instead of packed fp32 math, a deferred P store wait,
-// S(j+1) issued in two 64-key halves (N = 64 MMAs run at the N = 128 rate), and two threads per query row (16 softmax warps:
-// correct, 3.75 vs 3.13 ms). cuDNN's fused attention is 14-17 % ahead on the same tensors (profiles/r02_attention_comparators.json).
-template <bool P_TMEM>
+template <bool P_SMEM>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                  const __grid_constant__ CUtensorMap tmV, const AttParams p) {
-  using Cfg = AttCfg<P_TMEM>;
+  using Cfg = AttCfg<P_SMEM>;
   constexpr int NS = Cfg::NS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* q_full = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
-  uint64_t* kv_full = q_full + 1;
+  uint64_t* q_empty = q_full + 1;
+  uint64_t* kv_full = q_empty + 1;
   uint64_t* kv_empty = kv_full + NS;
-  uint64_t* s_full = kv_empty + NS;
-  uint64_t* p_half = s_full + 2;  // [X][half]: P columns [64*half, 64*half+64) of query tile X are in place
-  uint64_t* o_done = p_half + 4;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_done + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  // Work decomposition (see AttParams): every role decodes it again INSIDE its own branch from an opaque copy of
-  // blockIdx.x, so that none of these values stays live across the register-starved softmax loop.
-  auto decode = [&](int& unit, int& kv_begin, int& nkv) {
-    int bx = blockIdx.x;
-    asm volatile("" : "+r"(bx));
-    unit = bx;
-    kv_begin = 0;
-    nkv = p.nkv;
-    if (bx >= p.full_units) {  // KV segment of a tail unit; kv_begin is even: barrier parities follow the global tile index
-      const int r = bx - p.full_units;
-      unit = p.full_units + r / p.ns;
-      const int per = (((p.nkv + p.ns - 1) / p.ns) + 1) & ~1;
-      kv_begin = (r % p.ns) * per;
-      nkv = min(per, p.nkv - kv_begin);
-    }
-  };
+  // work decomposition (see AttParams)
+  int unit = blockIdx.x, kv_begin = 0, nkv = p.nkv;
+  if (static_cast<int>(blockIdx.x) >= p.full_units) {  // KV segment of a tail unit
+    const int r = blockIdx.x - p.full_units;
+    unit = p.full_units + r / p.ns;
+    const int per = (((p.nkv + p.ns - 1) / p.ns) + 1) & ~1;
+    kv_begin = (r % p.ns) * per;
+    nkv = min(per, p.nkv - kv_begin);
+  }
+  const int head = unit / p.nq;
+  const int q0 = (unit - head * p.nq) * 256;
+  const int nx = q0 + 128 < p.Lq ? 2 : 1;   // query tiles of this unit that hold rows < Lq
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
     mbar_init(q_full, 1);
+    mbar_init(q_empty, 8);
     for (int i = 0; i < NS; ++i) {
       mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&p_half[2 * i], 128);
-      mbar_init(&p_half[2 * i + 1], 128);
-      mbar_init(&o_done[i], 1);
+      mbar_init(&kv_empty[i], 8);   // one arrival per consumer warp
     }
     fence_barrier_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp < 4) {
-    setmaxnreg_dec<80>();
+    setmaxnreg_dec<40>();
     if (warp == 0 && lane == 0) {
       // ------------------------------- TMA producer -------------------------------
-      int unit, kv_begin, nkv;
-      decode(unit, kv_begin, nkv);
-      const int head = unit / p.nq;
-      const int q0 = (unit - head * p.nq) * 256;
-      mbar_arrive_expect_tx(q_full, 2 * ATT_TILE_BYTES);
-      for (int x = 0; x < 2; ++x)
+      int it = 0;
+      for (int X = 0; X < nx; ++X) {
+        if (X == 1) mbar_wait(q_empty, 0);
+        mbar_arrive_expect_tx(q_full, ATT_TILE_BYTES);
         for (int s = 0; s < 2; ++s)
-          tma_load_2d(smem + Cfg::Q_OFF + x * ATT_TILE_BYTES + s * 16384, &tmQ, q_full, head * 128 + s * 64,
-                      q0 + x * 128);
-      for (int it = 0; it < 2 * nkv; ++it) {
-        const int slot = it % NS;
-        const uint32_t ph = (it / NS) & 1;
-        mbar_wait(&kv_empty[slot], ph ^ 1);
-        mbar_arrive_expect_tx(&kv_full[slot], ATT_TILE_BYTES);
-        const CUtensorMap* tm = (it & 1) ? &tmV : &tmK;
-        uint8_t* dst = smem + Cfg::KV_OFF + slot * ATT_TILE_BYTES;
-        const int j = kv_begin + (it >> 1);
-        tma_load_2d(dst, tm, &kv_full[slot], head * 128, j * 128);
-        tma_load_2d(dst + 16384, tm, &kv_full[slot], head * 128 + 64, j * 128);
-      }
-    } else if (warp == 1 && lane == 0) {
-      // ------------------------------- MMA issuer -------------------------------
-      int unit, kv_begin, nkv;
-      decode(unit, kv_begin, nkv);
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_pv = make_idesc_bf16(128, 128, 0, 1);
-      const uint32_t sQ = smem_u32(smem + Cfg::Q_OFF);
-      const uint32_t sP = smem_u32(smem + Cfg::P_OFF);
-      const uint32_t sKV = smem_u32(smem + Cfg::KV_OFF);
-      // Descriptors differ only in their 14-bit start-address field; build the constant part once and add the
-      // (compile-time) tile offsets: one 64-bit add per operand per MMA keeps the issue loop short.
-      const uint64_t kdesc0 = make_smem_desc_sw128(0, 16, 1024);      // K-major tiles (Q, K, P-in-smem)
-      const uint64_t vdesc0 = make_smem_desc_sw128(0, 16384, 1024);   // MN-major V tile
-      // tile X of Q / P sits ATT_TILE_BYTES after tile 0: + X * (ATT_TILE_BYTES >> 4) in the address field (scalars, not
-      // arrays: an array indexed by X lands in local memory whenever the X loop is not unrolled)
-      const uint64_t qdesc0 = kdesc0 + (sQ >> 4);
-      const uint64_t pdesc0 = kdesc0 + (sP >> 4);
-      constexpr uint64_t kTileStep = ATT_TILE_BYTES >> 4;
-      auto issue_S = [&](int X, uint32_t kbase) {
-        const uint64_t kd = kdesc0 + (kbase >> 4);
-        uint64_t qd = qdesc0 + X * kTileStep;
-        asm volatile("" : "+l"(qd));   // opaque: keeps the 16 per-kk Q descriptors from being hoisted out of the KV loop
-#pragma unroll                         // (they do not fit next to the softmax branch's registers and would be spilled)
-        for (int kk = 0; kk < 8; ++kk) {
-          const uint32_t off16 = ((kk >> 2) * 16384 + (kk & 3) * 32) >> 4;
-          umma_ss(tmem_base + X * 128, qd + off16, kd + off16, idesc_s, kk != 0 ? 1u : 0u);
+          tma_load_2d(smem + Cfg::Q_OFF + s * 16384, &tmQ, q_full, head * 128 + s * 64, q0 + X * 128);
+        for (int jj = 0; jj < 2 * nkv; ++jj, ++it) {
+          const int slot = it % NS;
+          mbar_wait(&kv_empty[slot], ((it / NS) & 1) ^ 1);
+          mbar_arrive_expect_tx(&kv_full[slot], ATT_TILE_BYTES);
+          const CUtensorMap* tm = (jj & 1) ? &tmV : &tmK;
+          uint8_t* dst = smem + Cfg::KV_OFF + slot * ATT_TILE_BYTES;
+          const int j = kv_begin + (jj >> 1);
+          tma_load_2d(dst, tm, &kv_full[slot], head * 128, j * 128);
+          tma_load_2d(dst + 16384, tm, &kv_full[slot], head * 128 + 64, j * 128);
         }
-      };
-      auto issue_PV = [&](int X, uint32_t vbase, bool acc, int half) {
-        const uint64_t vd = vdesc0 + (vbase >> 4);
-#pragma unroll
-        for (int kq = 0; kq < 4; ++kq) {
-          const int kk = half * 4 + kq;
-          const uint64_t bdesc = vd + ((kk * 2048) >> 4);
-          if (P_TMEM) {
-            umma_ts(tmem_base + 256 + X * 128, tmem_base + X * 128 + kk * 8, bdesc, idesc_pv,
-                    (acc || kk != 0) ? 1u : 0u);
-          } else {
-            const uint32_t off16 = ((kk >> 2) * 16384 + (kk & 3) * 32) >> 4;
-            umma_ss(tmem_base + 256 + X * 128, pdesc0 + X * kTileStep + off16, bdesc, idesc_pv, (acc || kk != 0) ? 1u : 0u);
-          }
-        }
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[0], 0);
-      tc_fence_after();
-      issue_S(0, sKV);
-      umma_commit(&s_full[0]);
-      issue_S(1, sKV);
-      umma_commit(&s_full[1]);
-      umma_commit(&kv_empty[0]);
-      // Measured alternatives (profiles/README.md): an event-driven loop polling both tiles with mbarrier.test_wait
-      // was 30% slower (each probe costs ~150 cycles vs the ~60-cycle wake-up of the blocking try_wait); one issuer
-      // thread per query tile was 30% slower as well — the tiles drift into phase (both in softmax, then both in MMA)
-      // and lose the ping-pong this single in-order issuer enforces.
-      for (int j = 0; j < nkv; ++j) {
-        const int iv = 2 * j + 1, ik = 2 * j + 2;
-        const int slot_v = iv % NS, slot_k = ik % NS;
-        const bool has_next = (j + 1 < nkv);
-        mbar_wait(&kv_full[slot_v], (iv / NS) & 1);
-        if (has_next) mbar_wait(&kv_full[slot_k], (ik / NS) & 1);
-        tc_fence_after();
-        const uint32_t vbase = sKV + slot_v * ATT_TILE_BYTES;
-        const uint32_t kbase = sKV + slot_k * ATT_TILE_BYTES;
-#pragma unroll
-        for (int X = 0; X < 2; ++X) {
-          long long* tr = (p.trace != nullptr && blockIdx.x == 1 && j >= 16 && j < 48)
-                              ? p.trace + (j - 16) * 32 + 16 + X * 4 : nullptr;
-          if (tr) tr[0] = clock64();
-          mbar_wait(&p_half[2 * X], j & 1);
-          if (tr) tr[1] = clock64();
-          tc_fence_after();
-          issue_PV(X, vbase, j > 0, 0);             // keys 0..63 of the tile, while the softmax warps finish 64..127
-          mbar_wait(&p_half[2 * X + 1], j & 1);
-          tc_fence_after();
-          issue_PV(X, vbase, true, 1);
-          if (has_next) {
-            issue_S(X, kbase);
-            umma_commit(&s_full[X]);
-          } else {
-            umma_commit(&o_done[X]);
-          }
-          if (tr) tr[2] = clock64();
-        }
-        umma_commit(&kv_empty[slot_v]);
-        if (has_next) umma_commit(&kv_empty[slot_k]);
       }
     }
   } else {
-    // ------------------------------- softmax / correction / epilogue -------------------------------
-    setmaxnreg_inc<208>();  // 128*80 + 256*208 = 63488 <= 384*168 (the CTA's register pool)
-    const int X = (warp - 4) >> 2;
-    const int quad = warp & 3;
-    const int row_in_tile = quad * 32 + lane;
-    const uint32_t lane_off = static_cast<uint32_t>(quad * 32) << 16;
-    const uint32_t tS = tmem_base + lane_off + X * 128;
-    const uint32_t tO = tmem_base + lane_off + 256 + X * 128;
+    // ------------------------------- S, softmax, P V, epilogue -------------------------------
+    setmaxnreg_inc<232>();
+    const int wg = (warp >> 2) - 1;
+    const int q4 = lane >> 2, c2 = 2 * (lane & 3);   // fragment rows q4 / q4 + 8 of the warp's 16, columns 8g + c2, +1
+    const int row_a = wg * 64 + (warp & 3) * 16 + q4;   // tile row of fragment row a (row b = row_a + 8)
     const float sc = p.scale_log2;
-    float m_used = -INFINITY;
-    float l = 0.f;
-
-    int kv_begin, kv_end;
-    {
-      int unit, nkv;
-      decode(unit, kv_begin, nkv);
-      kv_end = kv_begin + nkv;
-    }
-    for (int j = kv_begin; j < kv_end; ++j) {   // global KV tile index (kv_begin is even: parity of j == local parity)
-      long long* tr = (p.trace != nullptr && blockIdx.x == 1 && (warp & 3) == 0 && lane == 0 && j >= 16 && j < 48)
-                          ? p.trace + (j - 16) * 32 + X * 8 : nullptr;
-      if (tr) tr[0] = clock64();
-      mbar_wait(&s_full[X], j & 1);
-      if (tr) tr[1] = clock64();
-      tc_fence_after();
-      const int kv_rem = p.Lk - j * 128;
-      if (kv_rem < 128) {
-        // last, partial KV tile (k_lens contract): overwrite the out-of-range columns of S with -inf in TMEM.
-        // Kept as a cold side-effecting loop so the per-element selects are not if-converted into every tile.
-#pragma unroll 1
-        for (int c = kv_rem >> 5; c < 4; ++c) {
-          uint32_t t[32];
-          tmem_ld32(tS + c * 32, t);
-          tmem_ld_wait();
+    const uint32_t sQ = smem_u32(smem + Cfg::Q_OFF) + wg * 64 * 128;
+    const uint32_t sP = smem_u32(smem + Cfg::P_OFF) + wg * 16384;
+    int it = 0;
+    for (int X = 0; X < nx; ++X) {
+      mbar_wait(q_full, X);
+      float o[64];
 #pragma unroll
-          for (int i = 0; i < 32; ++i)
-            if (c * 32 + i >= kv_rem) t[i] = 0xff800000u;  // -inf
-          tmem_st32(tS + c * 32, t);
+      for (int i = 0; i < 64; ++i) o[i] = 0.f;
+      float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows a / b: running max (log2 domain) and sum
+      for (int j = 0; j < nkv; ++j, it += 2) {
+        const int slot_k = it % NS, slot_v = (it + 1) % NS;
+        mbar_wait(&kv_full[slot_k], (it / NS) & 1);
+        const uint32_t sK = smem_u32(smem + Cfg::KV_OFF + slot_k * ATT_TILE_BYTES);
+        float s[64];
+#pragma unroll
+        for (int i = 0; i < 64; ++i) s[i] = 0.f;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {   // D = 128: two 64-column slabs, 4 k-steps of 32 B each
+          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
+          wgmma_ss_acc64<0>(s, make_smem_desc_sw128(sQ + off, 16, 1024), make_smem_desc_sw128(sK + off, 16, 1024), kk != 0);
         }
-        tmem_st_wait();
-      }
-      uint32_t s[4][32];
-      tmem_ld32(tS + 0, s[0]);
-      tmem_ld32(tS + 32, s[1]);
-      tmem_ld32(tS + 64, s[2]);
-      tmem_ld32(tS + 96, s[3]);
-      tmem_ld_wait();
-      if (tr) tr[2] = clock64();
-      // 8 independent running maxima (a single fmaxf chain is 128 dependent ops of 4-cycle latency each); ptxas pairs them into
-      // 64 FMNMX3
-      float mxa[8];
-#pragma unroll
-      for (int a = 0; a < 8; ++a) mxa[a] = -INFINITY;
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-#pragma unroll
-        for (int i = 0; i < 32; ++i) mxa[i & 7] = fmaxf(mxa[i & 7], __uint_as_float(s[c][i]));
-      const float mx = fmaxf(fmaxf(fmaxf(mxa[0], mxa[1]), fmaxf(mxa[2], mxa[3])),
-                             fmaxf(fmaxf(mxa[4], mxa[5]), fmaxf(mxa[6], mxa[7])));
-      const float ms = mx * sc;
-      if (tr) {
-        asm volatile("" ::"f"(ms));
-        tr[3] = clock64();
-      }
-      if (j == kv_begin) {
-        m_used = ms;
-      } else {
-        const bool need = ms > m_used + 8.0f;
-        if (__any_sync(0xffffffffu, need)) {
-          const float m_new = fmaxf(m_used, ms);
-          const float alpha = fast_exp2(m_used - m_new);
-          l *= alpha;
-#pragma unroll 1
-          for (int c = 0; c < 4; ++c) {
-            uint32_t o[32];
-            tmem_ld32(tO + c * 32, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st32(tO + c * 32, o);
-          }
-          tmem_st_wait();
-          m_used = m_new;
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(s);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&kv_empty[slot_k]);
+          if (j == nkv - 1) mbar_arrive(q_empty);   // the producer may load the next query tile
         }
-      }
-      // probabilities on packed fp32 pairs: one FFMA2 scales+shifts two scores, one FADD2 accumulates two sums
-      const uint64_t sc2 = f2_pack(sc, sc);
-      const uint64_t negm2 = f2_pack(-m_used, -m_used);
-      uint64_t ls2[2] = {0ull, 0ull};  // two independent packed partial row sums (0ull == (+0.f, +0.f))
+        const int kv_rem = p.Lk - (kv_begin + j) * 128;
+        if (kv_rem < 128) {   // last, partial KV tile (k_lens contract): columns past the end count as -inf
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        uint32_t pk[32];
-#pragma unroll
-        for (int i = 0; i < 32; ++i) {
-          const int c0 = h * 64 + 2 * i;
-          const uint64_t x2 = f2_fma(f2_pack(__uint_as_float(s[c0 >> 5][c0 & 31]),
-                                             __uint_as_float(s[(c0 + 1) >> 5][(c0 + 1) & 31])), sc2, negm2);
-          float x0, x1;
-          f2_unpack(x2, x0, x1);
-          const float p0 = fast_exp2(x0), p1 = fast_exp2(x1);
-          ls2[i & 1] = f2_add(ls2[i & 1], f2_pack(p0, p1));
-          pk[i] = pack_bf16x2(p0, p1);
+          for (int i = 0; i < 64; ++i)
+            if (8 * (i >> 2) + c2 + (i & 1) >= kv_rem) s[i] = -INFINITY;
         }
-        if (P_TMEM) {
-          tmem_st32(tS + h * 32, pk);
-          tmem_st_wait();
-        } else {
-          // K-major 128B-swizzled slab h of the P tile: row r, 16-byte chunk c -> r*128 + ((c ^ (r & 7)) << 4)
-          uint8_t* slab = smem + Cfg::P_OFF + X * ATT_TILE_BYTES + h * 16384 + row_in_tile * 128;
+        float mx0 = -INFINITY, mx1 = -INFINITY;
 #pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            uint4 w = make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-            *reinterpret_cast<uint4*>(slab + ((c ^ (row_in_tile & 7)) << 4)) = w;
+        for (int g = 0; g < 16; ++g) {
+          mx0 = fmaxf(mx0, fmaxf(s[4 * g], s[4 * g + 1]));
+          mx1 = fmaxf(mx1, fmaxf(s[4 * g + 2], s[4 * g + 3]));
+        }
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 1));
+        mx0 = fmaxf(mx0, __shfl_xor_sync(0xffffffffu, mx0, 2));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
+        mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
+        const float mn0 = fmaxf(m0, mx0 * sc), mn1 = fmaxf(m1, mx1 * sc);
+        const float al0 = fast_exp2(m0 - mn0), al1 = fast_exp2(m1 - mn1);   // 0 on the first tile (m = -inf)
+        m0 = mn0;
+        m1 = mn1;
+        l0 *= al0;
+        l1 *= al1;
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {
+          o[4 * g] *= al0;
+          o[4 * g + 1] *= al0;
+          o[4 * g + 2] *= al1;
+          o[4 * g + 3] *= al1;
+        }
+        // P as the A fragment of the k-steps of P V: k-step kk covers keys [16kk, 16kk + 16) = accumulator groups 2kk, 2kk + 1
+        uint32_t pa[8][4];
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          float e[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) e[i] = fast_exp2(s[8 * kk + i] * sc - ((i & 2) ? m1 : m0));
+          l0 += (e[0] + e[1]) + (e[4] + e[5]);
+          l1 += (e[2] + e[3]) + (e[6] + e[7]);
+          pa[kk][0] = pack_bf16x2(e[0], e[1]);   // row a, keys 2t, 2t+1
+          pa[kk][1] = pack_bf16x2(e[2], e[3]);   // row b
+          pa[kk][2] = pack_bf16x2(e[4], e[5]);   // row a, keys 8 + 2t, +1
+          pa[kk][3] = pack_bf16x2(e[6], e[7]);   // row b
+        }
+        if (P_SMEM) {
+          // K-major 128B-swizzled P of this warpgroup: slab = key / 64; row r, 16-byte chunk c -> r*128 + ((c ^ (r & 7)) << 4)
+          const int ra = row_a - wg * 64, rb = ra + 8;
+#pragma unroll
+          for (int kk = 0; kk < 8; ++kk) {
+            uint8_t* slab = smem + Cfg::P_OFF + wg * 16384 + (kk >> 2) * 8192;
+            const int k0 = (kk & 3) * 16 + c2, k1 = k0 + 8;   // key within the slab
+            *reinterpret_cast<uint32_t*>(slab + ra * 128 + (((k0 >> 3) ^ (ra & 7)) << 4) + (k0 & 7) * 2) = pa[kk][0];
+            *reinterpret_cast<uint32_t*>(slab + rb * 128 + (((k0 >> 3) ^ (rb & 7)) << 4) + (k0 & 7) * 2) = pa[kk][1];
+            *reinterpret_cast<uint32_t*>(slab + ra * 128 + (((k1 >> 3) ^ (ra & 7)) << 4) + (k1 & 7) * 2) = pa[kk][2];
+            *reinterpret_cast<uint32_t*>(slab + rb * 128 + (((k1 >> 3) ^ (rb & 7)) << 4) + (k1 & 7) * 2) = pa[kk][3];
           }
           fence_proxy_async_smem();
+          named_bar_sync(1 + wg, 128);
         }
-        if (tr) tr[4 + h] = clock64();
-        tc_fence_before();
-        mbar_arrive(&p_half[2 * X + h]);
+        mbar_wait(&kv_full[slot_v], ((it + 1) / NS) & 1);
+        const uint32_t sV = smem_u32(smem + Cfg::KV_OFF + slot_v * ATT_TILE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {   // V is MN-major: 16 keys = 2048 B further, D slabs 16 KB apart
+          const uint64_t vdesc = make_smem_desc_sw128(sV + kk * 2048, 16384, 1024);
+          if (P_SMEM)
+            wgmma_ss_acc64<1>(o, make_smem_desc_sw128(sP + (kk >> 2) * 8192 + (kk & 3) * 32, 16, 1024), vdesc, 1u);
+          else
+            wgmma_rs_n128_tb(o, pa[kk], vdesc, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(o);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&kv_empty[slot_v]);
       }
-      {
-        float a0, a1, b0, b1;
-        f2_unpack(ls2[0], a0, a1);
-        f2_unpack(ls2[1], b0, b1);
-        l += (a0 + a1) + (b0 + b1);
+      l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
+      l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
+      l1 += __shfl_xor_sync(0xffffffffu, l1, 2);
+
+      // epilogue: O / l -> bf16 -> global [Lq, heads*128] (or the KV-segment workspace / the owner rank's receive buffer)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {   // fragment row a, then row b
+        const int row_t = X * 128 + row_a + 8 * h;
+        const float m = h ? m1 : m0, l = h ? l1 : l0;
+        if (static_cast<int>(blockIdx.x) >= p.full_units) {
+          const long long prow = static_cast<long long>(blockIdx.x - p.full_units) * 256 + row_t;
+          float* wo = p.ws_o + prow * 128;
+#pragma unroll
+          for (int g = 0; g < 16; ++g) *reinterpret_cast<float2*>(wo + 8 * g + c2) = make_float2(o[4 * g + 2 * h], o[4 * g + 2 * h + 1]);
+          if ((lane & 3) == 0) *reinterpret_cast<float2*>(p.ws_ml + prow * 2) = make_float2(m, l);
+          continue;
+        }
+        const int q_row = q0 + row_t;
+        if (q_row >= p.Lq) continue;
+        __nv_bfloat16* orow = p.out + static_cast<long long>(q_row) * p.ldo + head * 128;
+        if (p.sp_world > 1) {
+          const int owner = q_row / p.sp_Lp;
+          const int t = q_row - owner * p.sp_Lp;
+          if (owner < p.sp_world)
+            orow = p.out_peers[owner] + (static_cast<long long>(p.sp_rank) * p.sp_Lp + t) * p.ldo + head * 128;
+        }
+        const float inv = 1.0f / l;
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {
+          uint32_t* dst = reinterpret_cast<uint32_t*>(orow + 8 * g + c2);
+          float v0 = o[4 * g + 2 * h] * inv, v1 = o[4 * g + 2 * h + 1] * inv;
+          if (p.accumulate) {
+            const float2 prev = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(dst));
+            v0 += prev.x;
+            v1 += prev.y;
+          }
+          *dst = pack_bf16x2(v0, v1);
+        }
       }
     }
-
-    // epilogue: O / l -> bf16 -> global [Lq, heads*128] (or the KV-segment workspace / the owner rank's receive buffer)
-    mbar_wait(&o_done[X], 0);
-    tc_fence_after();
-    {
-      int unit, kvb, nk;
-      decode(unit, kvb, nk);
-      attention_epilogue(p, tO, m_used, l, X, row_in_tile, unit);
-    }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -516,11 +336,11 @@ static size_t split_workspace_bytes(size_t ctas) { return ctas * 256 * 130 * siz
 static int g_debug_force_split = 0;   // yb_debug_force_split: tests force the KV split through paths that carry no flags
 
 // force_ns: 0 = automatic tail split, 1 = never, 2..4 = split EVERY unit into that many KV segments (tests)
-template <bool P_TMEM>
+template <bool P_SMEM>
 static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
                             AttParams p, int heads, cudaStream_t stream, int force_ns, void* ws, long long ws_bytes) {
-  using Cfg = AttCfg<P_TMEM>;
-  auto kern = attention_kernel<P_TMEM>;
+  using Cfg = AttCfg<P_SMEM>;
+  auto kern = attention_kernel<P_SMEM>;
   static bool attr_set[kMaxDevices] = {false};
   if (int rc = ensure_dynamic_smem(kern, Cfg::SMEM_BYTES, attr_set, "attention")) return rc;
   if (force_ns == 0 && g_debug_force_split >= 1 && g_debug_force_split <= 4) force_ns = g_debug_force_split;
@@ -528,7 +348,7 @@ static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, cons
   const int units = p.nq * heads;
   int tail = 0;
   p.ws_o = p.ws_ml = nullptr;
-  const bool allowed = !p.accumulate && p.trace == nullptr && ws != nullptr;
+  const bool allowed = !p.accumulate && ws != nullptr;
   attention_plan(units, p.nkv, sm_count(), allowed, force_ns, &p.full_units, &tail, &p.ns);
   if (tail > 0) {
     const size_t ctas = static_cast<size_t>(tail) * p.ns;
@@ -562,8 +382,8 @@ static int dispatch_attention(const void* q, long long ldq, const void* k, long 
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmV, v, p.Lk, cols, ldv, 128, 64);
   if (rc) return rc;
-  if (flags & YB_ATT_P_SMEM) return launch_attention<false>(tmQ, tmK, tmV, p, heads, stream, force_ns, ws, ws_bytes);
-  return launch_attention<true>(tmQ, tmK, tmV, p, heads, stream, force_ns, ws, ws_bytes);
+  if (flags & YB_ATT_P_SMEM) return launch_attention<true>(tmQ, tmK, tmV, p, heads, stream, force_ns, ws, ws_bytes);
+  return launch_attention<false>(tmQ, tmK, tmV, p, heads, stream, force_ns, ws, ws_bytes);
 }
 
 }  // namespace yb
@@ -609,7 +429,7 @@ extern "C" int yb_attention_ex(const void* q, long long ldq, const void* k, long
   p.Lk = Lk;
   p.nkv = (Lk + 127) / 128;
   p.accumulate = (flags & YB_ATT_ACCUMULATE) ? 1 : 0;
-  p.trace = static_cast<long long*>(trace);
+  (void)trace;   // accepted for ABI compatibility, ignored (see include/yume_b200.h)
   p.sp_world = 1;
   p.sp_rank = 0;
   p.sp_Lp = 0;
@@ -638,7 +458,6 @@ extern "C" int yb_attention_sp(const void* q, long long ldq, const void* k, long
   p.Lk = Lk;
   p.nkv = (Lk + 127) / 128;
   p.accumulate = 0;
-  p.trace = nullptr;
   p.scale_log2 = scale * 1.4426950408889634f;
   for (int i = 0; i < 8; ++i) p.out_peers[i] = i < world ? static_cast<__nv_bfloat16*>(out_peers[i]) : nullptr;
   p.sp_world = world;

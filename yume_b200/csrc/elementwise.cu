@@ -661,7 +661,7 @@ using namespace yb;
 extern "C" int yb_bcast_add(const void* a, const void* b, void* out, int R1, int R2, int n, void* stream_) {
   if (!a || !b || !out || R1 <= 0 || R2 <= 0 || n <= 0) return YB_ERR_ARG;
   const long long total = static_cast<long long>(R1) * R2 * n;
-  const int blocks = static_cast<int>(total / 256 + 1 < 148LL * 8 ? total / 256 + 1 : 148LL * 8);
+  const int blocks = static_cast<int>(total / 256 + 1 < static_cast<long long>(sm_count()) * 8 ? total / 256 + 1 : static_cast<long long>(sm_count()) * 8);
   bcast_add_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(a), static_cast<const float*>(b), static_cast<float*>(out), R1, R2, n);
   return check_launch("bcast_add");
@@ -790,7 +790,7 @@ extern "C" int yb_patchify(const void* x, long long sc, long long sf, long long 
   if (!x || !out || Cin <= 0 || F <= 0 || H <= 0 || W <= 0 || ph <= 0 || pw <= 0) return YB_ERR_ARG;
   const int Hp = (H + ph - 1) / ph, Wp = (W + pw - 1) / pw;
   const long long total = static_cast<long long>(F) * Hp * Wp * Cin * ph * pw;
-  const int blocks = static_cast<int>(total / 256 + 1 < 148LL * 16 ? total / 256 + 1 : 148LL * 16);
+  const int blocks = static_cast<int>(total / 256 + 1 < static_cast<long long>(sm_count()) * 16 ? total / 256 + 1 : static_cast<long long>(sm_count()) * 16);
   patchify_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(x), sc, sf, sh, sw, static_cast<__nv_bfloat16*>(out), ldo, Cin, F, H, W, ph, pw, Hp,
       Wp);
@@ -801,7 +801,7 @@ extern "C" int yb_unpatchify(const void* y, long long ldy, void* out, int Cout, 
                              void* stream_) {
   if (!y || !out || Cout <= 0 || F <= 0 || Hp <= 0 || Wp <= 0 || ph <= 0 || pw <= 0) return YB_ERR_ARG;
   const long long total = static_cast<long long>(Cout) * F * Hp * ph * Wp * pw;
-  const int blocks = static_cast<int>(total / 256 + 1 < 148LL * 16 ? total / 256 + 1 : 148LL * 16);
+  const int blocks = static_cast<int>(total / 256 + 1 < static_cast<long long>(sm_count()) * 16 ? total / 256 + 1 : static_cast<long long>(sm_count()) * 16);
   unpatchify_kernel<<<blocks, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(y), ldy, static_cast<float*>(out), Cout, F, Hp, Wp, ph, pw);
   return check_launch("unpatchify");

@@ -1,8 +1,8 @@
-// gemm.cu — persistent, warp-specialised tcgen05 GEMM for sm_100a with fused epilogues.
+// gemm.cu — persistent, warp-specialised wgmma GEMM for sm_90a (H100) with fused epilogues.
 //
 //   out[M,N] = epilogue( A[M,K] (bf16, row-major) x B[N,K]^T (bf16, row-major, i.e. nn.Linear.weight) + bias[N] )
 //
-// This is the B200-native replacement for every nn.Linear on the reference's denoise path
+// This is the H100-native replacement for every nn.Linear on the reference's denoise path
 // (reference: wan23/modules/model.py:171-174 q/k/v/o, :265-267 ffn, :455-457 text_embedding;
 //  wan/modules/model.py:282-287, 358-361, 436-438), with the elementwise work the reference runs as
 // separate eager kernels folded into the epilogue:
@@ -13,12 +13,12 @@
 //   YB_EPI_GATE_RES   resid_f32 += (acc + bias) * gate[tok[m], n]  (o-proj / ffn.2 + adaLN gate + residual add:
 //                                                                   model.py:304, 308, 312)
 //
-// Structure (one CTA per SM, 192 threads):
-//   warp 0      TMA producer: A tile 128x64 and B tile BLOCK_Nx64 (128B-swizzled) into a 4..6-stage smem ring
-//   warp 1      MMA issuer: tcgen05.mma cta_group::1 kind::f16, M=128, N=BLOCK_N, K=16 x4 per stage, fp32
-//               accumulators in TMEM, double-buffered (2 x BLOCK_N columns) so the epilogue of tile i overlaps
-//               the main loop of tile i+1
-//   warps 2..5  epilogue: tcgen05.ld 32x32b -> registers -> fused math -> global
+// Structure (one CTA per SM, 384 threads = 3 warpgroups):
+//   warpgroup 0     TMA producer (one thread): A tile 128x64 and B tile block_n x 64 (128B-swizzled) into an smem ring
+//   warpgroups 1-2  consumers: wgmma m64nNk16 over rows [64*(wg-1), +64) of the tile, fp32 accumulators in registers,
+//                   then the fused epilogue (registers -> per-warp smem transpose -> full row segments to global)
+// The SM-pair form (CLUSTER = 2) is a cluster of two CTAs that owns a 256 x block_n tile: each CTA loads its own 128 rows of A
+// and HALF of the B tile, and multicasts that half into both CTAs, so the B operand crosses L2 once per pair of SMs.
 #include "yb_host.h"
 #include "yb_ptx.cuh"
 
@@ -26,8 +26,12 @@ namespace yb {
 
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_THREADS = 384;
 constexpr int GEMM_GROUP_N = 8;   // rasterisation: n-tiles per group (keeps A and B footprints L2 resident)
+constexpr int GEMM_MAX_STAGES = 8;
+constexpr int GEMM_SMEM_BYTES = 227 * 1024;                 // the H100 per-block maximum
+constexpr int GEMM_A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
+constexpr int GEMM_EPI_STAGE_BYTES = 8 * 16 * 36 * 4;       // 8 consumer warps x 16 rows x 36 floats
 
 struct GemmParams {
   int M, N, K;
@@ -54,7 +58,7 @@ struct GemmParams {
   int st_t, st_h, st_w;         // conv stride per axis (1 or 2): the tensor map samples every st-th voxel (elementStrides), so a box
                                 // still lands as 128 dense rows; cT/cH/cW are OUTPUT extents, the tile origin scales by the stride
   int num_m_tiles, num_n_tiles;
-  int block_n, stages;          // SM-pair kernel (gemm_pair_kernel): runtime N tile (multiple of 32, <= 256) and ring depth
+  int block_n, stages;          // N tile (multiple of 32, <= 256) and smem ring depth
   // Tail split-K of the SM-pair kernel (GATE_RES launches): work items [0, sk_full) are whole tiles; item sk_full + u is K segment
   // u % sk_ns (sk_per 64-column blocks) of tile sk_full + u / sk_ns and leaves its raw fp32 accumulator in sk_ws[u][256][block_n]
   // for gemm_splitk_combine_kernel. sk_ns == 1: no split (sk_full == number of tiles).
@@ -79,20 +83,15 @@ constexpr int CONVW_ROWS = GEMM_BLOCK_M + 2;
 constexpr int CONVW_A_SLAB = 17 * 1024;  // 130 rows x 128 B = 16640 B, padded to the 1024-B swizzle pattern
 constexpr int CONVW_A_STAGES = 4;
 
-template <int BLOCK_N, int CONVW = 0>
-struct GemmCfg {
-  static constexpr int A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-  static constexpr int B_BYTES = BLOCK_N * GEMM_BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = CONVW ? B_BYTES : A_BYTES + B_BYTES;   // CONVW: the ring holds B tiles only
-  static constexpr int STAGES = (BLOCK_N == 256) ? 4 : 6;
-  static constexpr int A_STAGES = CONVW ? CONVW_A_STAGES : 0;
-  static constexpr int A_RING_OFF = STAGES * STAGE_BYTES;
-  static constexpr int BAR_OFF = A_RING_OFF + A_STAGES * CONVW_A_SLAB;
-  static constexpr int STAGE_OFF = BAR_OFF + 256;                // epilogue transpose buffers: 4 warps x 32 x 36 floats
-  static constexpr int SMEM_BYTES = STAGE_OFF + 4 * 32 * 36 * 4 + 1024 /*align slack*/;
-  static constexpr int TMEM_COLS = 2 * BLOCK_N;  // 512 or 256: power of two
-  static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
-};
+// smem: [stages x (A tile | B tile)] [CONVW A ring] [epilogue transpose buffers] [barriers]. The B tile is allocated in whole
+// 64-row slabs (the N = 64 MMAs of an odd block_n read the rows past block_n; their columns are never stored).
+__host__ __device__ constexpr int gemm_b_bytes(int block_n) { return ((block_n + 63) / 64) * 64 * GEMM_BLOCK_K * 2; }
+__host__ __device__ constexpr int gemm_stage_bytes(int block_n, int convw) { return (convw ? 0 : GEMM_A_BYTES) + gemm_b_bytes(block_n); }
+__host__ __device__ constexpr int gemm_a_ring_bytes(int convw) { return convw ? CONVW_A_STAGES * CONVW_A_SLAB : 0; }
+static int gemm_stages(int block_n, int convw) {
+  const int s = (GEMM_SMEM_BYTES - 1024 - 256 - GEMM_EPI_STAGE_BYTES - gemm_a_ring_bytes(convw)) / gemm_stage_bytes(block_n, convw);
+  return s > GEMM_MAX_STAGES ? GEMM_MAX_STAGES : s;
+}
 
 __device__ __forceinline__ void tile_coords(int tile, int num_m_tiles, int num_n_tiles, int& m_tile, int& n_tile) {
   const int per_group = GEMM_GROUP_N * num_m_tiles;
@@ -104,432 +103,182 @@ __device__ __forceinline__ void tile_coords(int tile, int num_m_tiles, int num_n
   n_tile = n_first + (r - m_tile * n_in_group);
 }
 
-// One 32-column chunk of an output tile: r = the accumulator row of tile row `lane` (TMEM lane), my_row / my_tok = logical output
-// row and gate-table row of that tile row (-1 = none). TMEM -> registers (lane = row) -> per-warp smem transpose (row pitch 36
-// floats: conflict-free for both the row-per-lane writes and the row-segment reads) -> fused math -> global, so that every global
-// access is a full 64/128-byte row segment shared by 4/8 adjacent lanes instead of 32 different rows per instruction.
+// One 32-column chunk of the 16 tile rows of a consumer warp, already transposed into `stage` (row pitch 36 floats) by the
+// caller. Lane l (< 16) holds my_row / my_tok = logical output row and gate-table row of the warp's tile row l (-1 = none).
+// Every global access is a full 64/128-byte row segment shared by 4/8 adjacent lanes.
 template <int EPI>
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const uint32_t (&r)[32], int col0, int my_row, int my_tok,
-                                               float* stage, int lane, float* sq = nullptr) {
+__device__ __forceinline__ void epilogue_rows16(const GemmParams& p, int col0, int my_row, int my_tok, const float* stage, int lane,
+                                                float* sq) {
   constexpr bool kBf16Out = (EPI == YB_EPI_BF16 || EPI == YB_EPI_GELU_BF16 || EPI == YB_EPI_GELU_ERF_BF16 ||
                              EPI == YB_EPI_RES_BF16 || EPI == YB_EPI_SP_QKV);
-  float4* st = reinterpret_cast<float4*>(stage + lane * 36);
+  if (col0 >= p.N) return;
+  if (kBf16Out) {
+    const int cq = (lane & 3) * 8;  // this lane's 8 columns of the 32-column chunk
+    float b[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (p.bias) {
+      const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq));
+      const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq + 4));
+      b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+    }
+    // optional N-split output (Ulysses layout): column block j of width n_split goes to out + j*split_stride
+    long long col_off = col0 + cq;
+    if (p.n_split > 0) col_off = static_cast<long long>(col0 / p.n_split) * p.split_stride + (col0 % p.n_split) + cq;
+    __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(p.out) + col_off;
+    long long ld = p.ldo;
+    if (EPI == YB_EPI_SP_QKV) {   // destination = the owner rank's receive buffer; rows are (this rank, local token)
+      const int part = col0 / p.sp_C, cin = col0 - part * p.sp_C;
+      const int peer = cin / p.sp_Wh;
+      ld = 3LL * p.sp_Wh;
+      obase = p.sp_peers[peer] + static_cast<long long>(p.sp_rank) * p.sp_Lp * ld + part * p.sp_Wh + (cin - peer * p.sp_Wh) + cq;
+    }
+    uint4 resv[2];
+    if (EPI == YB_EPI_RES_BF16) {  // residual loads first (they may alias the stores for all the compiler knows)
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
-    st[i] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                        __uint_as_float(r[4 * i + 3]));
-  __syncwarp();
-  if (col0 < p.N) {
-    if (kBf16Out) {
-      const int cq = (lane & 3) * 8;  // this lane's 8 columns of the 32-column chunk
-      float b[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-      if (p.bias) {
-        const float4 b0 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq));
-        const float4 b1 = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq + 4));
-        b[0] = b0.x; b[1] = b0.y; b[2] = b0.z; b[3] = b0.w; b[4] = b1.x; b[5] = b1.y; b[6] = b1.z; b[7] = b1.w;
+      for (int it = 0; it < 2; ++it) {
+        const int rowi = __shfl_sync(0xffffffffu, my_row, it * 8 + (lane >> 2));
+        resv[it] = make_uint4(0u, 0u, 0u, 0u);
+        if (rowi >= 0) resv[it] = *reinterpret_cast<const uint4*>(p.res + static_cast<long long>(rowi) * p.res_ld + col0 + cq);
       }
-      // optional N-split output (Ulysses layout): column block j of width n_split goes to out + j*split_stride
-      long long col_off = col0 + cq;
-      if (p.n_split > 0) col_off = static_cast<long long>(col0 / p.n_split) * p.split_stride + (col0 % p.n_split) + cq;
-      __nv_bfloat16* obase = reinterpret_cast<__nv_bfloat16*>(p.out) + col_off;
-      long long sp_ld = p.ldo;
-      if (EPI == YB_EPI_SP_QKV) {   // destination = the owner rank's receive buffer; rows are (this rank, local token)
-        const int part = col0 / p.sp_C, cin = col0 - part * p.sp_C;
-        const int peer = cin / p.sp_Wh;
-        sp_ld = 3LL * p.sp_Wh;
-        obase = p.sp_peers[peer] + static_cast<long long>(p.sp_rank) * p.sp_Lp * sp_ld + part * p.sp_Wh + (cin - peer * p.sp_Wh) + cq;
-      }
-      uint4 resv[4];
-      if (EPI == YB_EPI_RES_BF16) {  // residual loads first (they may alias the stores for all the compiler knows)
+    }
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
-          const int rowi = __shfl_sync(0xffffffffu, my_row, it * 8 + (lane >> 2));
-          resv[it] = make_uint4(0u, 0u, 0u, 0u);
-          if (rowi >= 0)
-            resv[it] = *reinterpret_cast<const uint4*>(p.res + static_cast<long long>(rowi) * p.res_ld + col0 + cq);
+    for (int it = 0; it < 2; ++it) {
+      const int rr = it * 8 + (lane >> 2);
+      const int rowi = __shfl_sync(0xffffffffu, my_row, rr);
+      const float4 a0 = *reinterpret_cast<const float4*>(stage + rr * 36 + cq);
+      const float4 a1 = *reinterpret_cast<const float4*>(stage + rr * 36 + cq + 4);
+      float v[8] = {a0.x + b[0], a0.y + b[1], a0.z + b[2], a0.w + b[3], a1.x + b[4], a1.y + b[5], a1.z + b[6], a1.w + b[7]};
+      if (EPI == YB_EPI_GELU_BF16) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = gelu_tanh(v[i]);
+      }
+      if (EPI == YB_EPI_GELU_ERF_BF16) {
+#pragma unroll
+        for (int i = 0; i < 8; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.7071067811865476f));
+      }
+      if (EPI == YB_EPI_RES_BF16) {
+        const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&resv[it]);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const float2 f = __bfloat1622float2(rh[i]);
+          v[2 * i] += f.x;
+          v[2 * i + 1] += f.y;
         }
       }
-#pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int rr = it * 8 + (lane >> 2);
-        const int rowi = __shfl_sync(0xffffffffu, my_row, rr);
-        const float4 a0 = *reinterpret_cast<const float4*>(stage + rr * 36 + cq);
-        const float4 a1 = *reinterpret_cast<const float4*>(stage + rr * 36 + cq + 4);
-        float v[8] = {a0.x + b[0], a0.y + b[1], a0.z + b[2], a0.w + b[3],
-                      a1.x + b[4], a1.y + b[5], a1.z + b[6], a1.w + b[7]};
-        if (EPI == YB_EPI_GELU_BF16) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = gelu_tanh(v[i]);
-        }
-        if (EPI == YB_EPI_GELU_ERF_BF16) {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) v[i] = 0.5f * v[i] * (1.0f + erff(v[i] * 0.7071067811865476f));
-        }
-        if (EPI == YB_EPI_RES_BF16) {
-          const __nv_bfloat162* rh = reinterpret_cast<const __nv_bfloat162*>(&resv[it]);
+      if (rowi >= 0) {
+        uint4 w;
+        w.x = pack_bf16x2(v[0], v[1]);
+        w.y = pack_bf16x2(v[2], v[3]);
+        w.z = pack_bf16x2(v[4], v[5]);
+        w.w = pack_bf16x2(v[6], v[7]);
+        *reinterpret_cast<uint4*>(obase + static_cast<long long>(rowi) * ld) = w;
+        if (EPI == YB_EPI_SP_QKV) {   // sum of squares of the ROUNDED values (what the receiver normalises)
+          const __nv_bfloat162* wh = reinterpret_cast<const __nv_bfloat162*>(&w);
+          float acc = 0.f;
 #pragma unroll
           for (int i = 0; i < 4; ++i) {
-            const float2 f = __bfloat1622float2(rh[i]);
-            v[2 * i] += f.x;
-            v[2 * i + 1] += f.y;
+            const float2 f = __bfloat1622float2(wh[i]);
+            acc += f.x * f.x + f.y * f.y;
           }
+          sq[it] += acc;
         }
-        if (rowi >= 0) {
-          uint4 w;
-          w.x = pack_bf16x2(v[0], v[1]);
-          w.y = pack_bf16x2(v[2], v[3]);
-          w.z = pack_bf16x2(v[4], v[5]);
-          w.w = pack_bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(obase + static_cast<long long>(rowi) * (EPI == YB_EPI_SP_QKV ? sp_ld : p.ldo)) = w;
-          if (EPI == YB_EPI_SP_QKV) {   // sum of squares of the ROUNDED values (what the receiver normalises)
-            const __nv_bfloat162* wh = reinterpret_cast<const __nv_bfloat162*>(&w);
-            float acc = 0.f;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              const float2 f = __bfloat1622float2(wh[i]);
-              acc += f.x * f.x + f.y * f.y;
-            }
-            sq[it] += acc;
-          }
-        }
-      }
-    } else {
-      const int cq = (lane & 7) * 4;  // this lane's 4 columns
-      float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (p.bias) b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq));
-      float* obase = reinterpret_cast<float*>(p.out) + col0 + cq;
-      // all loads first, then all stores: the residual rows may alias as far as the compiler can tell, so a
-      // load placed after a store would serialise one L2 round trip per row
-      float4 xv[8], gv[8];
-      int rowv[8];
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + (lane >> 3);
-        const int tok = __shfl_sync(0xffffffffu, my_tok, rr);
-        rowv[it] = __shfl_sync(0xffffffffu, my_row, rr);
-        xv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-        gv[it] = make_float4(1.f, 1.f, 1.f, 1.f);
-        if (EPI == YB_EPI_GATE_RES && rowv[it] >= 0) {
-          xv[it] = *reinterpret_cast<const float4*>(obase + static_cast<long long>(rowv[it]) * p.ldo);
-          if (p.gate)
-            gv[it] = __ldg(reinterpret_cast<const float4*>(p.gate + static_cast<long long>(tok) * p.gate_ld + col0 + cq));
-        }
-      }
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + (lane >> 3);
-        float4 a = *reinterpret_cast<const float4*>(stage + rr * 36 + cq);
-        a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
-        if (rowv[it] >= 0) {
-          float4* o4 = reinterpret_cast<float4*>(obase + static_cast<long long>(rowv[it]) * p.ldo);
-          if (EPI == YB_EPI_F32) {
-            *o4 = a;
-          } else {  // YB_EPI_GATE_RES
-            float4 x = xv[it];
-            x.x += a.x * gv[it].x; x.y += a.y * gv[it].y; x.z += a.z * gv[it].z; x.w += a.w * gv[it].w;
-            *o4 = x;
-          }
-        }
-      }
-    }
-  }
-}
-
-template <int BLOCK_N, int EPI, int CONVW = 0>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
-  using Cfg = GemmCfg<BLOCK_N, CONVW>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* a_full = empty_bar + Cfg::STAGES;          // CONVW only (A_STAGES == 0 otherwise)
-  uint64_t* a_empty = a_full + Cfg::A_STAGES;
-  uint64_t* tmem_full = a_empty + Cfg::A_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;
-  const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&tmA);
-    tma_prefetch_desc(&tmB);
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < Cfg::A_STAGES; ++i) {
-      mbar_init(&a_full[i], 1);
-      mbar_init(&a_empty[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 128);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  if (warp == 0) {
-    // ------------------------------- TMA producer -------------------------------
-    if (CONVW && lane == 0) {
-      int stage = 0, a_stage = 0;
-      uint32_t phase = 0, a_phase = 0;
-      const int groups = num_kb / 3;                      // (dt, dh, channel chunk)
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_tile, n_tile;
-        tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
-        const int per_t = p.tiles_h * p.tiles_w;
-        const int it = m_tile / per_t, rem = m_tile - it * per_t;
-        const int ih = rem / p.tiles_w, iw = rem - ih * p.tiles_w;
-        for (int g = 0; g < groups; ++g) {
-          const int tdh = g / p.cin_chunks, cc = g - tdh * p.cin_chunks;
-          const int dt = tdh / p.kh, dh = tdh - dt * p.kh;
-          mbar_wait(&a_empty[a_stage], a_phase ^ 1);
-          mbar_arrive_expect_tx(&a_full[a_stage], CONVW_ROWS * GEMM_BLOCK_K * 2);
-          tma_load_4d(smem + Cfg::A_RING_OFF + a_stage * CONVW_A_SLAB, &tmA, &a_full[a_stage], cc * GEMM_BLOCK_K,
-                      iw * GEMM_BLOCK_M - p.off_w, ih + dh - p.off_h, it + dt - p.off_t);
-          if (++a_stage == Cfg::A_STAGES) {
-            a_stage = 0;
-            a_phase ^= 1;
-          }
-#pragma unroll 1
-          for (int dw = 0; dw < 3; ++dw) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            mbar_arrive_expect_tx(&full_bar[stage], Cfg::B_BYTES);
-            tma_load_2d(smem + stage * Cfg::STAGE_BYTES, &tmB, &full_bar[stage],
-                        ((tdh * 3 + dw) * p.cin_chunks + cc) * GEMM_BLOCK_K, n_tile * BLOCK_N);
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-        }
-      }
-    } else if (!CONVW && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        int m_tile, n_tile;
-        tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          mbar_arrive_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          // A goes through a 3-D map [chunk, row, col]: logical column k lives in chunk k / a_split (one chunk when
-          // the operand is an ordinary matrix; P chunks for the Ulysses-received attention output)
-          const int kcol = kb * GEMM_BLOCK_K;
-          if (p.conv) {
-            // tap (dt, dh, dw) reads padded voxel (t + dt, h + dh, w + dw): P[tp][hp][wp] = X[max(tp-2,0)][clamp(hp-1)]
-            // [clamp(wp-1)] — temporal pad 2 in front only (causal), replicate everywhere
-            const int tap = kb / p.cin_chunks, cc = kb - tap * p.cin_chunks;
-            const int dt = tap / (p.kh * p.kw), dh = (tap / p.kw) % p.kh, dw = tap % p.kw;
-            const int per_t = p.tiles_h * p.tiles_w;
-            const int it = m_tile / per_t, rem = m_tile - it * per_t;
-            const int ih = rem / p.tiles_w, iw = rem - ih * p.tiles_w;
-            tma_load_4d(sa, &tmA, &full_bar[stage], cc * GEMM_BLOCK_K, iw * p.TW * p.st_w + dw - p.off_w,
-                        ih * p.TH * p.st_h + dh - p.off_h, it * p.TT * p.st_t + dt - p.off_t);
-          } else {
-            const int chunk = kcol / p.a_split;
-            tma_load_3d(sa, &tmA, &full_bar[stage], kcol - chunk * p.a_split, m_tile * GEMM_BLOCK_M, chunk);
-          }
-          tma_load_2d(sb, &tmB, &full_bar[stage], kb * GEMM_BLOCK_K, n_tile * BLOCK_N);
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ------------------------------- MMA issuer -------------------------------
-    if (CONVW && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BLOCK_M, BLOCK_N, 0, 0);
-      int stage = 0, a_stage = 0;
-      uint32_t phase = 0, a_phase = 0;
-      int local = 0;
-      const int groups = num_kb / 3;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int acc = local & 1;
-        const uint32_t acc_phase = (local >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int g = 0; g < groups; ++g) {
-          mbar_wait(&a_full[a_stage], a_phase);
-          const uint32_t sa = smem_u32(smem + Cfg::A_RING_OFF + a_stage * CONVW_A_SLAB);
-#pragma unroll 1
-          for (int dw = 0; dw < 3; ++dw) {
-            mbar_wait(&full_bar[stage], phase);
-            tc_fence_after();
-            const uint64_t adesc = make_smem_desc_sw128(sa + dw * 128, 16, 1024);   // tap dw = rows [dw, dw + 128)
-            const uint64_t bdesc = make_smem_desc_sw128(smem_u32(smem + stage * Cfg::STAGE_BYTES), 16, 1024);
-#pragma unroll
-            for (int k = 0; k < GEMM_BLOCK_K / 16; ++k)
-              umma_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (g | dw | k) != 0 ? 1u : 0u);
-            umma_commit(&empty_bar[stage]);
-            if (++stage == Cfg::STAGES) {
-              stage = 0;
-              phase ^= 1;
-            }
-          }
-          umma_commit(&a_empty[a_stage]);
-          if (++a_stage == Cfg::A_STAGES) {
-            a_stage = 0;
-            a_phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
-      }
-    } else if (!CONVW && lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(GEMM_BLOCK_M, BLOCK_N, 0, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int local = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-        const int acc = local & 1;
-        const uint32_t acc_phase = (local >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * BLOCK_N;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-          const uint64_t adesc = make_smem_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(sb, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
-            // advance 16 elements (32 B) along K inside the 128B swizzle atom: +2 in the (addr>>4) field
-            umma_ss(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(&tmem_full[acc]);
       }
     }
   } else {
-    // ------------------------------- epilogue warps -------------------------------
-    // TMEM -> registers (lane = row) -> per-warp smem transpose (row pitch 36 floats: conflict-free for both the
-    // row-per-lane writes and the row-segment reads) -> global, so that every global access is a full 64/128-byte
-    // row segment shared by 4/8 adjacent lanes instead of 32 different rows per instruction.
-    const int quad = warp & 3;  // TMEM lane quadrant this warp may access
-    float* stage = reinterpret_cast<float*>(smem + Cfg::STAGE_OFF) + quad * (32 * 36);
-    int local = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++local) {
-      int m_tile, n_tile;
-      tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
-      const int acc = local & 1;
-      const uint32_t acc_phase = (local >> 1) & 1;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * BLOCK_N;
-      // logical output row of tile row (quad*32 + lane): the matrix row, or the voxel index of a conv tile; -1 = none
-      int my_row;
-      {
-        const int r = quad * 32 + lane;
-        if (p.conv) {
-          const int per_t = p.tiles_h * p.tiles_w;
-          const int it = m_tile / per_t, rem = m_tile - it * per_t;
-          const int ih = rem / p.tiles_w, iw = rem - ih * p.tiles_w;
-          const int tw = r % p.TW, th = (r / p.TW) % p.TH, tt = r / (p.TW * p.TH);
-          const int t = it * p.TT + tt, h = ih * p.TH + th, w = iw * p.TW + tw;
-          my_row = (t < p.cT && h < p.cH && w < p.cW) ? ((t * p.out_t_mul + p.out_t_add) * p.cH + h) * p.cW + w : -1;
-        } else {
-          const int row = m_tile * GEMM_BLOCK_M + r;
-          my_row = row < p.M ? row : -1;
+    const int cq = (lane & 7) * 4;  // this lane's 4 columns
+    float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
+    if (p.bias) b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq));
+    float* obase = reinterpret_cast<float*>(p.out) + col0 + cq;
+    // all loads first, then all stores: the residual rows may alias as far as the compiler can tell, so a
+    // load placed after a store would serialise one L2 round trip per row
+    float4 xv[4], gv[4];
+    int rowv[4];
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const int rr = it * 4 + (lane >> 3);
+      const int tok = __shfl_sync(0xffffffffu, my_tok, rr);
+      rowv[it] = __shfl_sync(0xffffffffu, my_row, rr);
+      xv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
+      gv[it] = make_float4(1.f, 1.f, 1.f, 1.f);
+      if (EPI == YB_EPI_GATE_RES && rowv[it] >= 0) {
+        xv[it] = *reinterpret_cast<const float4*>(obase + static_cast<long long>(rowv[it]) * p.ldo);
+        if (p.gate) gv[it] = __ldg(reinterpret_cast<const float4*>(p.gate + static_cast<long long>(tok) * p.gate_ld + col0 + cq));
+      }
+    }
+#pragma unroll
+    for (int it = 0; it < 4; ++it) {
+      const int rr = it * 4 + (lane >> 3);
+      float4 a = *reinterpret_cast<const float4*>(stage + rr * 36 + cq);
+      a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+      if (rowv[it] >= 0) {
+        float4* o4 = reinterpret_cast<float4*>(obase + static_cast<long long>(rowv[it]) * p.ldo);
+        if (EPI == YB_EPI_F32) {
+          *o4 = a;
+        } else {  // YB_EPI_GATE_RES
+          float4 x = xv[it];
+          x.x += a.x * gv[it].x; x.y += a.y * gv[it].y; x.z += a.z * gv[it].z; x.w += a.w * gv[it].w;
+          *o4 = x;
         }
       }
-      if (EPI == YB_EPI_GATE_RES && my_row >= 0) {
-        // The residual rows of this tile are cold in HBM and the 4 epilogue warps keep too few bytes in flight to pull
-        // them at speed: prefetch them into L2 while the accumulator of this tile is still being computed.
-        const char* xrow = reinterpret_cast<const char*>(reinterpret_cast<const float*>(p.out) +
-                                                         static_cast<long long>(my_row) * p.ldo + n_tile * BLOCK_N);
-        const int ncols = min(BLOCK_N, p.N - n_tile * BLOCK_N);
-        for (int b = 0; b < ncols * 4; b += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(xrow + b));
-      }
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      int my_tok = 0;  // gate-table row of tile row `lane`
-      if (EPI == YB_EPI_GATE_RES && p.gate != nullptr && p.tok_idx != nullptr && my_row >= 0)
-        my_tok = p.tok_idx[my_row];
-#pragma unroll 1
-      for (int c = 0; c < BLOCK_N / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld32(t_row + c * 32, r);
-        tmem_ld_wait();
-        epilogue_chunk<EPI>(p, r, n_tile * BLOCK_N + c * 32, my_row, my_tok, stage, lane);
-        __syncwarp();
-      }
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[acc]);
     }
   }
+}
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+// one 64-wide K block of this warpgroup's 64 x block_n accumulator: 4 k-steps of 16 (32 B inside the 128-B swizzle row).
+// NM = MMA width: 256 / 128 (block_n equal to it) or 64 (any multiple of 32: block_n / 64 rounded up N = 64 MMAs). A compile-time
+// choice: with the three forms in one kernel ptxas serialises the wgmma pipeline.
+template <int NM>
+__device__ __forceinline__ void gemm_mma_k64(float (&acc)[128], uint32_t sa, uint32_t sb, int block_n, bool zero_first) {
+  const uint64_t ad0 = make_smem_desc_sw128(sa, 16, 1024), bd0 = make_smem_desc_sw128(sb, 16, 1024);
+  const int nb64 = (block_n + 63) >> 6;
+#pragma unroll
+  for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) {
+    const uint64_t ad = ad0 + 2 * k, bd = bd0 + 2 * k;
+    const uint32_t accum = (zero_first && k == 0) ? 0u : 1u;
+    if (NM == 256) {
+      wgmma_ss_n256<0>(acc, ad, bd, accum);
+    } else if (NM == 128) {
+      wgmma_ss_n128<0>(acc, ad, bd, accum);
+    } else {   // 64-column slabs of the B tile sit 8 KB apart
+      wgmma_ss_n64<0>(acc, ad, bd, accum);
+      if (nb64 > 1) wgmma_ss_n64<32>(acc, ad, bd + (8192 >> 4), accum);
+      if (nb64 > 2) wgmma_ss_n64<64>(acc, ad, bd + (16384 >> 4), accum);
+      if (nb64 > 3) wgmma_ss_n64<96>(acc, ad, bd + (24576 >> 4), accum);
+    }
   }
 }
 
-// ------------------------------------------------------------------------------------------------------------------------
-// SM-pair GEMM (`tcgen05.mma.cta_group::2`): a cluster of two CTAs owns one 256 x block_n output tile. CTA r of the pair holds rows
-// [r*128, r*128+128) of the tile (its own A rows, its own accumulator lanes) and stages HALF of the B tile; one MMA instruction
-// issued by the leader CTA multiplies 256 x block_n x 16 across both SMs, so each SM fetches 16 KB + block_n*64 B of operands per
-// 64-wide k-step instead of 16 KB + block_n*128 B — the operand fetch from shared memory is what holds 1-CTA MMAs below the math
-// rate (profiles/README.md). Measured on the DiT shapes: 1474-1505 TFLOP/s against 1381-1408 for the 1-CTA kernel (cuBLAS, which
-// pairs SMs too: 1534-1665), results bit-identical (profiles/r02_gemm_pair.md).
-//   warp 0      TMA producer (both CTAs): own 128x64 A tile + own half of the B tile per k-step; completion bytes of BOTH CTAs are
-//               credited to the LEADER's full barrier (2-SM TMA form)
-//   warp 1      MMA issuer (leader CTA only): M = 256, N = block_n, K = 16 x4 per stage; commits are multicast to both CTAs'
-//               empty / tmem_full barriers
-//   warps 2..5  epilogue (both CTAs): own 128 rows, the same fused epilogues as the 1-CTA kernel; they arrive on the LEADER's
-//               tmem_empty barrier (count 256)
-// block_n is a RUNTIME multiple of 32 (<= 256): the host picks the N tile that minimises waves x tile width on the 74 SM pairs
-// (M = 2310 x N = 3072, the 8-GPU o-projection: 120 tiles of 256x256 are 1.62 waves; 140 tiles of 256x224 fill two waves exactly
-// 12.5 % sooner). Accumulators are double buffered at TMEM columns 0 and 256.
-// ------------------------------------------------------------------------------------------------------------------------
-constexpr int PAIR_EPI_STAGE_BYTES = 4 * 32 * 36 * 4;
-constexpr int PAIR_MAX_STAGES = 8;
-__host__ __device__ constexpr int pair_stage_bytes(int block_n) { return GEMM_BLOCK_M * GEMM_BLOCK_K * 2 + (block_n / 2) * GEMM_BLOCK_K * 2; }
-__host__ __device__ constexpr int pair_bar_off(int block_n, int stages) { return stages * pair_stage_bytes(block_n); }
-__host__ __device__ constexpr int pair_smem_bytes(int block_n, int stages) {
-  return pair_bar_off(block_n, stages) + 256 + PAIR_EPI_STAGE_BYTES + 1024;
+template <int CLUSTER>
+__device__ __forceinline__ void release_slot(uint64_t* bar, int lane) {
+  __syncwarp();
+  if (lane == 0) {
+    if (CLUSTER == 1) {
+      mbar_arrive(bar);
+    } else {   // the slot is refilled by BOTH CTAs' multicasts: free it in both
+      mbar_arrive_cluster(bar, 0);
+      mbar_arrive_cluster(bar, 1);
+    }
+  }
 }
 
-template <int EPI>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+template <int EPI, int CONVW, int CLUSTER, int NM>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  static_assert(!(CONVW && CLUSTER != 1), "the kw-fused conv runs on single CTAs");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int block_n = p.block_n, stages = p.stages;
-  const int stage_bytes = pair_stage_bytes(block_n);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + pair_bar_off(block_n, stages));   // used in the leader CTA only
-  uint64_t* empty_bar = full_bar + PAIR_MAX_STAGES;
-  uint64_t* tmem_full = empty_bar + PAIR_MAX_STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;                                                     // used in the leader CTA only
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
+  const int stage_bytes = gemm_stage_bytes(block_n, CONVW);
+  uint8_t* a_ring = smem + stages * stage_bytes;
+  float* epi = reinterpret_cast<float*>(a_ring + gemm_a_ring_bytes(CONVW));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi) + GEMM_EPI_STAGE_BYTES);
+  uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
+  uint64_t* a_full = empty_bar + GEMM_MAX_STAGES;   // CONVW only
+  uint64_t* a_empty = a_full + CONVW_A_STAGES;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int rank = static_cast<int>(cluster_ctarank());
-  const int tile_first = blockIdx.x >> 1, tile_step = gridDim.x >> 1;
-  const int num_tiles = p.num_m_tiles * p.num_n_tiles;            // tiles of 256 x block_n
+  const int rank = CLUSTER == 2 ? static_cast<int>(cluster_ctarank()) : 0;
+  const int tile_first = blockIdx.x / CLUSTER, tile_step = gridDim.x / CLUSTER;
+  const int num_tiles = p.num_m_tiles * p.num_n_tiles;   // tiles of (128 * CLUSTER) x block_n
   const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
   const int num_work = p.sk_full + (num_tiles - p.sk_full) * p.sk_ns;   // == num_tiles without a split tail
   // work item -> (tile, K-block range, partial slot or -1); every role walks the same sequence
@@ -543,250 +292,261 @@ gemm_pair_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       part = u;
     }
   };
+  // conv tile -> origin of its TT x TH x TW output box
+  auto conv_box = [&](int mt, int& it, int& ih, int& iw) {
+    const int per_t = p.tiles_h * p.tiles_w;
+    it = mt / per_t;
+    const int rem = mt - it * per_t;
+    ih = rem / p.tiles_w;
+    iw = rem - ih * p.tiles_w;
+  };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
+      mbar_init(&empty_bar[i], 8 * CLUSTER);   // every consumer warp of every CTA that writes into the slot
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 256);   // 4 epilogue warps of each CTA of the pair
+    for (int i = 0; i < (CONVW ? CONVW_A_STAGES : 0); ++i) {
+      mbar_init(&a_full[i], 1);
+      mbar_init(&a_empty[i], 8);
     }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc_2cta(tmem_ptr, 512);   // same warp and same smem slot in both CTAs
-  tc_fence_before();
   __syncthreads();
-  cluster_sync_all();                               // every barrier of the pair exists before any remote signal
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  if (CLUSTER > 1) cluster_sync_all();   // every barrier of the pair exists before any remote signal
 
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ------------------------------- TMA producer -------------------------------
+      int stage = 0, a_stage = 0;
+      uint32_t phase = 0, a_phase = 0;
       for (int w = tile_first; w < num_work; w += tile_step) {
         int tile, kb0, kb1, part, m_tile, n_tile;
         decode_work(w, tile, kb0, kb1, part);
         tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * stage_bytes;
-          if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 2 * stage_bytes);
-          const int kcol = kb * GEMM_BLOCK_K;
-          if (p.conv) {   // implicit-GEMM conv: this CTA's 128-voxel box of tap (dt, dh, dw), channel chunk cc (see gemm_kernel)
-            const int tap = kb / p.cin_chunks, cc = kb - tap * p.cin_chunks;
-            const int dt = tap / (p.kh * p.kw), dh = (tap / p.kw) % p.kh, dw = tap % p.kw;
-            const int mt = m_tile * 2 + rank, per_t = p.tiles_h * p.tiles_w;
-            const int it = mt / per_t, rem = mt - it * per_t;
-            const int ih = rem / p.tiles_w, iw = rem - ih * p.tiles_w;
-            tma_load_4d_2cta(sa, &tmA, &full_bar[stage], cc * GEMM_BLOCK_K, iw * p.TW * p.st_w + dw - p.off_w,
-                             ih * p.TH * p.st_h + dh - p.off_h, it * p.TT * p.st_t + dt - p.off_t);   // (a pair's second box past the last tile is all out of bounds: zeros)
-          } else {
-            const int chunk = kcol / p.a_split;      // K-split A (Ulysses receive buffer): see the 1-CTA producer
-            tma_load_3d_2cta(sa, &tmA, &full_bar[stage], kcol - chunk * p.a_split, (m_tile * 2 + rank) * GEMM_BLOCK_M, chunk);
-          }
-          tma_load_2d_2cta(sa + GEMM_BLOCK_M * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kcol,
-                           n_tile * block_n + rank * (block_n / 2));
-          if (++stage == stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      const uint32_t idesc = make_idesc_bf16(256, block_n, 0, 0);
-      int stage = 0, local = 0;
-      uint32_t phase = 0;
-      for (int w = tile_first; w < num_work; w += tile_step, ++local) {
-        int tile, kb0, kb1, part;
-        decode_work(w, tile, kb0, kb1, part);
-        const int acc = local & 1;
-        mbar_wait_cluster(&tmem_empty[acc], ((local >> 1) & 1) ^ 1);   // arrivals come from both CTAs
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
-          const uint64_t adesc = make_smem_desc_sw128(sa, 16, 1024);
-          const uint64_t bdesc = make_smem_desc_sw128(sa + GEMM_BLOCK_M * GEMM_BLOCK_K * 2, 16, 1024);
-#pragma unroll
-          for (int k = 0; k < GEMM_BLOCK_K / 16; ++k) umma_ss_2cta(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, ((kb - kb0) | k) != 0);
-          umma_commit_2cta(&empty_bar[stage]);        // frees the slot in BOTH CTAs
-          if (++stage == stages) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit_2cta(&tmem_full[acc]);            // accumulator ready in BOTH CTAs
-      }
-    }
-  } else {
-    const int quad = warp & 3;
-    float* stage = reinterpret_cast<float*>(smem + pair_bar_off(block_n, stages) + 256) + quad * (32 * 36);
-    int local = 0;
-    for (int w = tile_first; w < num_work; w += tile_step, ++local) {
-      int tile, kb0, kb1, part, m_tile, n_tile;
-      decode_work(w, tile, kb0, kb1, part);
-      tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
-      const int acc = local & 1;
-      const uint32_t t_row = tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + acc * 256;
-      if (part >= 0) {
-        // K segment of a split tail tile: the raw fp32 accumulator goes to the workspace, row-major [256][block_n]; the fused
-        // epilogue runs in gemm_splitk_combine_kernel over the sum of the segments
-        float* wrow = p.sk_ws + (static_cast<long long>(part) * 256 + rank * GEMM_BLOCK_M + quad * 32 + lane) * block_n;
-        mbar_wait(&tmem_full[acc], (local >> 1) & 1);
-        tc_fence_after();
-#pragma unroll 1
-        for (int c = 0; c < block_n / 32; ++c) {
-          uint32_t r[32];
-          tmem_ld32(t_row + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            *reinterpret_cast<uint4*>(wrow + c * 32 + 4 * i) = make_uint4(r[4 * i], r[4 * i + 1], r[4 * i + 2], r[4 * i + 3]);
-        }
-        tc_fence_before();
-        mbar_arrive_leader(&tmem_empty[acc]);
-        continue;
-      }
-      int my_row;
-      if (p.conv) {   // tile row -> voxel of this CTA's TT x TH x TW box -> output row (see gemm_kernel)
-        const int r = quad * 32 + lane, mt = m_tile * 2 + rank, per_t = p.tiles_h * p.tiles_w;
-        const int it = mt / per_t, rem = mt - it * per_t;
-        const int ih = rem / p.tiles_w, iw = rem - ih * p.tiles_w;
-        const int tw = r % p.TW, th = (r / p.TW) % p.TH, tt = r / (p.TW * p.TH);
-        const int t = it * p.TT + tt, hh = ih * p.TH + th, ww = iw * p.TW + tw;
-        my_row = (t < p.cT && hh < p.cH && ww < p.cW) ? ((t * p.out_t_mul + p.out_t_add) * p.cH + hh) * p.cW + ww : -1;
-      } else {
-        const int row = (m_tile * 2 + rank) * GEMM_BLOCK_M + quad * 32 + lane;
-        my_row = row < p.M ? row : -1;
-      }
-      const int ncols = min(block_n, p.N - n_tile * block_n);
-      if (EPI == YB_EPI_GATE_RES && my_row >= 0) {   // pull the (cold) residual rows of this tile into L2 under the main loop
-        const char* xrow = reinterpret_cast<const char*>(reinterpret_cast<const float*>(p.out) +
-                                                         static_cast<long long>(my_row) * p.ldo + n_tile * block_n);
-        for (int b = 0; b < ncols * 4; b += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(xrow + b));
-      }
-      int my_tok = 0;
-      if (EPI == YB_EPI_GATE_RES && p.gate != nullptr && p.tok_idx != nullptr && my_row >= 0) my_tok = p.tok_idx[my_row];
-      if constexpr (EPI == YB_EPI_GATE_RES) {
-        // x += (acc + bias) * gate, software-pipelined: the residual / gate operands of chunk c+1 are in flight while chunk c is
-        // read from TMEM, transposed and stored, and those of chunk 0 are requested BEFORE the accumulator is waited for. With
-        // one or two tiles per CTA (the 8-GPU shapes) no later main loop hides this epilogue: at M = 2310 the un-pipelined form
-        // ran the o-projection at 623 TFLOP/s against 1003 with a plain bf16 store.
-        const int cq = (lane & 7) * 4;
-        int rowv[8], tokv[8];
-#pragma unroll
-        for (int it = 0; it < 8; ++it) {
-          const int rr = it * 4 + (lane >> 3);
-          rowv[it] = __shfl_sync(0xffffffffu, my_row, rr);
-          tokv[it] = __shfl_sync(0xffffffffu, my_tok, rr);
-        }
-        float4 xc[8], gc[8], xn[8], gn[8];
-        auto fetch = [&](int col0, float4 (&xv)[8], float4 (&gv)[8]) {
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            xv[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-            gv[it] = make_float4(1.f, 1.f, 1.f, 1.f);
-            if (rowv[it] >= 0 && col0 < p.N) {
-              xv[it] = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.out) + static_cast<long long>(rowv[it]) * p.ldo + col0 + cq);
-              if (p.gate)
-                gv[it] = __ldg(reinterpret_cast<const float4*>(p.gate + static_cast<long long>(tokv[it]) * p.gate_ld + col0 + cq));
+        if (CONVW) {
+          int it, ih, iw;
+          conv_box(m_tile, it, ih, iw);
+          const int groups = num_kb / 3;   // (dt, dh, channel chunk)
+          for (int g = 0; g < groups; ++g) {
+            const int tdh = g / p.cin_chunks, cc = g - tdh * p.cin_chunks;
+            const int dt = tdh / p.kh, dh = tdh - dt * p.kh;
+            mbar_wait(&a_empty[a_stage], a_phase ^ 1);
+            mbar_arrive_expect_tx(&a_full[a_stage], CONVW_ROWS * GEMM_BLOCK_K * 2);
+            tma_load_4d(a_ring + a_stage * CONVW_A_SLAB, &tmA, &a_full[a_stage], cc * GEMM_BLOCK_K, iw * GEMM_BLOCK_M - p.off_w,
+                        ih + dh - p.off_h, it + dt - p.off_t);
+            if (++a_stage == CONVW_A_STAGES) {
+              a_stage = 0;
+              a_phase ^= 1;
             }
-          }
-        };
-        fetch(n_tile * block_n, xc, gc);
-        mbar_wait(&tmem_full[acc], (local >> 1) & 1);
-        tc_fence_after();
 #pragma unroll 1
-        for (int c = 0; c < block_n / 32; ++c) {
-          const int col0 = n_tile * block_n + c * 32;
-          if (c + 1 < block_n / 32) fetch(col0 + 32, xn, gn);
-          uint32_t r[32];
-          tmem_ld32(t_row + c * 32, r);
-          tmem_ld_wait();
-          float4* st = reinterpret_cast<float4*>(stage + lane * 36);
-#pragma unroll
-          for (int i = 0; i < 8; ++i)
-            st[i] = make_float4(__uint_as_float(r[4 * i]), __uint_as_float(r[4 * i + 1]), __uint_as_float(r[4 * i + 2]),
-                                __uint_as_float(r[4 * i + 3]));
-          __syncwarp();
-          if (col0 < p.N) {
-            float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias) b = __ldg(reinterpret_cast<const float4*>(p.bias + col0 + cq));
-#pragma unroll
-            for (int it = 0; it < 8; ++it) {
-              const int rr = it * 4 + (lane >> 3);
-              float4 a = *reinterpret_cast<const float4*>(stage + rr * 36 + cq);
-              if (rowv[it] >= 0) {
-                float4 x = xc[it];
-                x.x += (a.x + b.x) * gc[it].x; x.y += (a.y + b.y) * gc[it].y; x.z += (a.z + b.z) * gc[it].z; x.w += (a.w + b.w) * gc[it].w;
-                *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + static_cast<long long>(rowv[it]) * p.ldo + col0 + cq) = x;
+            for (int dw = 0; dw < 3; ++dw) {
+              mbar_wait(&empty_bar[stage], phase ^ 1);
+              mbar_arrive_expect_tx(&full_bar[stage], block_n * GEMM_BLOCK_K * 2);
+              tma_load_2d(smem + stage * stage_bytes, &tmB, &full_bar[stage], ((tdh * 3 + dw) * p.cin_chunks + cc) * GEMM_BLOCK_K,
+                          n_tile * block_n);
+              if (++stage == stages) {
+                stage = 0;
+                phase ^= 1;
               }
             }
           }
-          __syncwarp();
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            xc[it] = xn[it];
-            gc[it] = gn[it];
+          continue;
+        }
+        for (int kb = kb0; kb < kb1; ++kb) {
+          if (CLUSTER > 1) mbar_wait_cluster(&empty_bar[stage], phase ^ 1);
+          else mbar_wait(&empty_bar[stage], phase ^ 1);
+          uint8_t* sa = smem + stage * stage_bytes;
+          uint8_t* sb = sa + GEMM_A_BYTES;
+          mbar_arrive_expect_tx(&full_bar[stage], GEMM_A_BYTES + block_n * GEMM_BLOCK_K * 2);
+          const int kcol = kb * GEMM_BLOCK_K;
+          const int mt = m_tile * CLUSTER + rank;   // this CTA's 128-row block (a pair's second block past the end is all zeros)
+          if (p.conv) {
+            // tap (dt, dh, dw) reads padded voxel (t + dt, h + dh, w + dw): P[tp][hp][wp] = X[max(tp-2,0)][clamp(hp-1)]
+            // [clamp(wp-1)] — temporal pad 2 in front only (causal), replicate everywhere
+            const int tap = kb / p.cin_chunks, cc = kb - tap * p.cin_chunks;
+            const int dt = tap / (p.kh * p.kw), dh = (tap / p.kw) % p.kh, dw = tap % p.kw;
+            int it, ih, iw;
+            conv_box(mt, it, ih, iw);
+            tma_load_4d(sa, &tmA, &full_bar[stage], cc * GEMM_BLOCK_K, iw * p.TW * p.st_w + dw - p.off_w,
+                        ih * p.TH * p.st_h + dh - p.off_h, it * p.TT * p.st_t + dt - p.off_t);
+          } else {
+            // A goes through a 3-D map [chunk, row, col]: logical column k lives in chunk k / a_split (one chunk when
+            // the operand is an ordinary matrix; P chunks for the Ulysses-received attention output)
+            const int chunk = kcol / p.a_split;
+            tma_load_3d(sa, &tmA, &full_bar[stage], kcol - chunk * p.a_split, mt * GEMM_BLOCK_M, chunk);
+          }
+          if (CLUSTER == 1) {
+            tma_load_2d(sb, &tmB, &full_bar[stage], kcol, n_tile * block_n);
+          } else {
+            const int half = block_n / 2;
+            tma_load_2d_multicast(sb + rank * half * GEMM_BLOCK_K * 2, &tmB, &full_bar[stage], kcol, n_tile * block_n + rank * half,
+                                  static_cast<uint16_t>(3));
+          }
+          if (++stage == stages) {
+            stage = 0;
+            phase ^= 1;
           }
         }
-        tc_fence_before();
-        mbar_arrive_leader(&tmem_empty[acc]);
+      }
+    }
+  } else {
+    // ------------------------------- consumers: MMA + epilogue -------------------------------
+    setmaxnreg_inc<232>();   // 128 x 40 + 256 x 232 <= 65536
+    const int wg = (warp >> 2) - 1;   // rows [64 * wg, +64) of the CTA's 128-row tile
+    const int r0 = wg * 64 + (warp & 3) * 16;   // first of the 16 tile rows this warp stores
+    float* stage_buf = epi + (warp - 4) * (16 * 36);
+    int stage = 0, a_stage = 0;
+    uint32_t phase = 0, a_phase = 0;
+    float acc[128];
+#pragma unroll
+    for (int i = 0; i < 128; ++i) acc[i] = 0.f;
+    for (int w = tile_first; w < num_work; w += tile_step) {
+      int tile, kb0, kb1, part, m_tile, n_tile;
+      decode_work(w, tile, kb0, kb1, part);
+      tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
+      const int mt = m_tile * CLUSTER + rank;
+      // logical output row of tile row r0 + (lane & 15): the matrix row, or the voxel index of a conv tile; -1 = none
+      int my_row;
+      {
+        const int r = r0 + (lane & 15);
+        if (p.conv) {
+          int it, ih, iw;
+          conv_box(mt, it, ih, iw);
+          const int tw = r % p.TW, th = (r / p.TW) % p.TH, tt = r / (p.TW * p.TH);
+          const int t = it * p.TT + tt, h = ih * p.TH + th, ww = iw * p.TW + tw;
+          my_row = (t < p.cT && h < p.cH && ww < p.cW) ? ((t * p.out_t_mul + p.out_t_add) * p.cH + h) * p.cW + ww : -1;
+        } else {
+          const int row = mt * GEMM_BLOCK_M + r;
+          my_row = row < p.M ? row : -1;
+        }
+      }
+      if (EPI == YB_EPI_GATE_RES && part < 0 && my_row >= 0 && lane < 16) {
+        // the residual rows of this tile are cold in HBM: pull them into L2 while the accumulator is computed
+        const char* xrow = reinterpret_cast<const char*>(reinterpret_cast<const float*>(p.out) +
+                                                         static_cast<long long>(my_row) * p.ldo + n_tile * block_n);
+        const int ncols = min(block_n, p.N - n_tile * block_n);
+        for (int b = 0; b < ncols * 4; b += 128) asm volatile("prefetch.global.L2 [%0];" ::"l"(xrow + b));
+      }
+      // main loop: wgmma groups of one stage stay in flight while the next stage is issued; a slot is released once the
+      // MMAs that read it have completed
+      int prev = -1;
+      if (CONVW) {
+        int prev_a = -1;
+        const int groups = num_kb / 3;
+        for (int g = 0; g < groups; ++g) {
+          mbar_wait(&a_full[a_stage], a_phase);
+          const uint32_t sa = smem_u32(a_ring + a_stage * CONVW_A_SLAB) + wg * 64 * 128;
+#pragma unroll 1
+          for (int dw = 0; dw < 3; ++dw) {
+            mbar_wait(&full_bar[stage], phase);
+            fence_regs(acc);
+            wgmma_fence();
+            gemm_mma_k64<NM>(acc, sa + dw * 128, smem_u32(smem + stage * stage_bytes), block_n, g == 0 && dw == 0);   // tap dw = rows [dw, dw + 128)
+            wgmma_commit();
+            wgmma_wait<1>();
+            fence_regs(acc);
+            if (prev >= 0) release_slot<1>(&empty_bar[prev], lane);
+            if (dw == 0 && prev_a >= 0) {
+              release_slot<1>(&a_empty[prev_a], lane);
+              prev_a = -1;
+            }
+            prev = stage;
+            if (++stage == stages) {
+              stage = 0;
+              phase ^= 1;
+            }
+          }
+          prev_a = a_stage;
+          if (++a_stage == CONVW_A_STAGES) {
+            a_stage = 0;
+            a_phase ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (prev >= 0) release_slot<1>(&empty_bar[prev], lane);
+        if (prev_a >= 0) release_slot<1>(&a_empty[prev_a], lane);
+      } else {
+        for (int kb = kb0; kb < kb1; ++kb) {
+          mbar_wait(&full_bar[stage], phase);
+          const uint32_t sa = smem_u32(smem + stage * stage_bytes);
+          fence_regs(acc);
+          wgmma_fence();
+          gemm_mma_k64<NM>(acc, sa + wg * 64 * 128, sa + GEMM_A_BYTES, block_n, kb == kb0);
+          wgmma_commit();
+          wgmma_wait<1>();
+          fence_regs(acc);
+          if (prev >= 0) release_slot<CLUSTER>(&empty_bar[prev], lane);
+          prev = stage;
+          if (++stage == stages) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+        wgmma_wait<0>();
+        fence_regs(acc);
+        if (prev >= 0) release_slot<CLUSTER>(&empty_bar[prev], lane);
+      }
+
+      const int q4 = lane >> 2, c2 = 2 * (lane & 3);   // fragment: rows q4 / q4 + 8, columns 8g + c2, +1
+      if (part >= 0) {
+        // K segment of a split tail tile: the raw fp32 accumulator goes to the workspace, row-major [256][block_n]; the fused
+        // epilogue runs in gemm_splitk_combine_kernel over the sum of the segments
+        float* wbase = p.sk_ws + (static_cast<long long>(part) * 256 + rank * GEMM_BLOCK_M + r0) * block_n;
+#pragma unroll
+        for (int g = 0; g < 32; ++g) {
+          if (g * 8 < block_n) {
+            *reinterpret_cast<float2*>(wbase + q4 * block_n + g * 8 + c2) = make_float2(acc[4 * g], acc[4 * g + 1]);
+            *reinterpret_cast<float2*>(wbase + (q4 + 8) * block_n + g * 8 + c2) = make_float2(acc[4 * g + 2], acc[4 * g + 3]);
+          }
+        }
         continue;
       }
-      mbar_wait(&tmem_full[acc], (local >> 1) & 1);
-      tc_fence_after();
-      float sq[4] = {0.f, 0.f, 0.f, 0.f};   // SP_QKV: running sum of squares of tile rows it*8 + lane/4 over the current part
-      auto flush_sq = [&](int part) {       // 4 lanes share a row: reduce, one atomic per row and (tile, part)
+      int my_tok = 0;  // gate-table row of tile row r0 + lane
+      if (EPI == YB_EPI_GATE_RES && p.gate != nullptr && p.tok_idx != nullptr && my_row >= 0) my_tok = p.tok_idx[my_row];
+      float sq[2] = {0.f, 0.f};   // SP_QKV: running sum of squares of warp rows it*8 + lane/4 over the current part
+      auto flush_sq = [&](int part_) {   // 4 lanes share a row: reduce, one atomic per row and (tile, part)
 #pragma unroll
-        for (int it = 0; it < 4; ++it) {
+        for (int it = 0; it < 2; ++it) {
           float v = sq[it];
           v += __shfl_xor_sync(0xffffffffu, v, 1);
           v += __shfl_xor_sync(0xffffffffu, v, 2);
           const int rowi = __shfl_sync(0xffffffffu, my_row, it * 8 + (lane >> 2));
-          if ((lane & 3) == 0 && rowi >= 0 && part < 2) atomicAdd(p.sp_sums + rowi * 2 + part, v);
+          if ((lane & 3) == 0 && rowi >= 0 && part_ < 2) atomicAdd(p.sp_sums + rowi * 2 + part_, v);
           sq[it] = 0.f;
         }
       };
       int cur_part = (EPI == YB_EPI_SP_QKV) ? (n_tile * block_n) / p.sp_C : 0;
-#pragma unroll 1
-      for (int c = 0; c < block_n / 32; ++c) {
-        uint32_t r[32];
-        tmem_ld32(t_row + c * 32, r);
-        tmem_ld_wait();
-        const int col0 = n_tile * block_n + c * 32;
-        if (EPI == YB_EPI_SP_QKV && col0 < p.N) {
-          const int part = col0 / p.sp_C;
-          if (part != cur_part) {
-            flush_sq(cur_part);
-            cur_part = part;
+#pragma unroll
+      for (int c = 0; c < 8; ++c) {
+        if (c * 32 < block_n) {
+#pragma unroll
+          for (int g = 0; g < 4; ++g) {
+            const int i = 4 * (4 * c + g);
+            *reinterpret_cast<float2*>(stage_buf + q4 * 36 + g * 8 + c2) = make_float2(acc[i], acc[i + 1]);
+            *reinterpret_cast<float2*>(stage_buf + (q4 + 8) * 36 + g * 8 + c2) = make_float2(acc[i + 2], acc[i + 3]);
           }
+          __syncwarp();
+          const int col0 = n_tile * block_n + c * 32;
+          if (EPI == YB_EPI_SP_QKV && col0 < p.N) {
+            const int pt = col0 / p.sp_C;
+            if (pt != cur_part) {
+              flush_sq(cur_part);
+              cur_part = pt;
+            }
+          }
+          epilogue_rows16<EPI>(p, col0, my_row, my_tok, stage_buf, lane, sq);
+          __syncwarp();
         }
-        epilogue_chunk<EPI>(p, r, col0, my_row, my_tok, stage, lane, sq);
-        __syncwarp();
       }
       if (EPI == YB_EPI_SP_QKV) flush_sq(cur_part);
-      tc_fence_before();
-      mbar_arrive_leader(&tmem_empty[acc]);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, 512);
-  }
+  if (CLUSTER > 1) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
 
 // Fused epilogue of the split tail tiles (YB_EPI_GATE_RES): x[row, col] += (sum of the K-segment partials + bias[col]) * gate[tok, col],
@@ -827,10 +587,11 @@ __global__ void __launch_bounds__(256) gemm_splitk_combine_kernel(const GemmPara
 
 // Tail split-K plan (host arithmetic, exported through yb_gemm_splitk_plan): `tiles` output tiles on `clusters` SM pairs leave a
 // last wave of r = tiles % clusters tiles; cutting each of them into ns K segments costs ceil(r * ns / clusters) sub-waves, each
-// 1 / ns of a tile plus a fixed ~6 us (pipeline fill + fp32 dump of the partial; a 64-column K block takes ~0.4 us, so 15 / num_kb
-// of a tile), plus the combine launch (13.6 / num_kb) and 1 % per segment of workspace traffic. Calibrated on
-// profiles/r02_gemm_splitk.md: 4-GPU FFN-down (228 tiles, K = 14336) 338 -> 305 us, 4-GPU o-projection 89 -> 86 us; the 8-GPU
-// FFN-down (120 tiles, 46 in the tail) gains 1 % with 3 segments and is left alone; never at 1 or 2 GPUs (full last waves).
+// 1 / ns of a tile plus a fixed 5 / num_kb of a tile (pipeline fill + fp32 dump of the partial, ~5 K blocks of 64 columns at the
+// ~1.8 us an SM pair spends per K block), plus the combine launch (6 / num_kb) and 1 % per segment of workspace traffic.
+// Calibrated on one H100 SXM (700 W), x += (A W^T + b) * gate, N = 3072, unsplit -> best split, us: M = 4620, K = 3072
+// 349 -> 327 (2 segments); M = 4620, K = 14336 1460 -> 1405 (2); M = 1500, K = 3072 175 -> 117 (6); M = 2310 at K = 3072 and
+// 14336 (54 tail tiles: two sub-waves) only lose, 184 -> 201 and 742 -> 785. The model picks each of these.
 static void gemm_splitk_plan(int tiles, int num_kb, int clusters, int force_ns, int* full, int* ns, int* per) {
   *full = tiles; *ns = 1; *per = num_kb;
   if (clusters <= 0 || force_ns == 1) return;
@@ -844,7 +605,7 @@ static void gemm_splitk_plan(int tiles, int num_kb, int clusters, int force_ns, 
     double best = 0.85;
     for (int n = 2; n <= 12 && num_kb / n >= 8; ++n) {
       const int pr = (num_kb + n - 1) / n;
-      const double cost = static_cast<double>((r * n + clusters - 1) / clusters) * (pr + 15.0) / num_kb + 13.6 / num_kb + 0.01 * n;
+      const double cost = static_cast<double>((r * n + clusters - 1) / clusters) * (pr + 5.0) / num_kb + 6.0 / num_kb + 0.01 * n;
       if (cost < best) { best = cost; *ns = n; }
     }
     if (*ns == 1) return;
@@ -855,24 +616,21 @@ static void gemm_splitk_plan(int tiles, int num_kb, int clusters, int force_ns, 
   *full = tiles - r;
 }
 
-// N tile of the SM-pair kernel: 256 (N itself, rounded up to 32, for narrower outputs). The kernel takes any multiple of 32 and
-// a waves-x-width cost model was tried: on the 8-GPU o-projection (M = 2310, N = 3072) 224-wide tiles fill two waves exactly
-// where 256-wide ones need 1.62, but measured 0.045 ms vs 0.043 ms (ffn1: 0.196 vs 0.176): narrower MMAs and more B re-reads cost
-// more than the idle tail (profiles/r02_gemm_pair.md). Host arithmetic only — exported through yb_gemm_plan.
+// N tile of the SM-pair kernel: 256, or N itself rounded up to 32 for narrower outputs. Host arithmetic only — exported through
+// yb_gemm_plan.
 static int pair_block_n(int M, int N, int clusters) {
   (void)M;
   (void)clusters;
   return N >= 256 ? 256 : ((N + 31) / 32) * 32;
 }
 
-// CTA pairs the device holds at once (GPCs with an odd SM count leave an SM unpaired): asked of the driver, SM count / 2 if the
-// query is unavailable
+// CTA pairs the device holds at once: asked of the driver, SM count / 2 if the query is unavailable
 template <typename Kern>
 static int pair_max_clusters(Kern kern) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(2 * (sm_count() / 2));
   cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = 227 * 1024;
+  cfg.dynamicSmemBytes = GEMM_SMEM_BYTES;
   cudaLaunchAttribute attr;
   attr.id = cudaLaunchAttributeClusterDimension;
   attr.val.clusterDim.x = 2;
@@ -888,25 +646,29 @@ static int pair_max_clusters(Kern kern) {
   return n;
 }
 
-template <int EPI>
-static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream, int split_k = 1,
-                            void* ws = nullptr, long long ws_bytes = 0) {
-  auto kern = gemm_pair_kernel<EPI>;
-  static bool attr_set[kMaxDevices] = {false};
-  if (int rc = ensure_dynamic_smem(kern, 227 * 1024, attr_set, "gemm_pair")) return rc;
-  p.num_m_tiles = p.conv ? (p.num_m_tiles + 1) / 2 : (p.M + 255) / 256;   // conv: pairs of 128-voxel boxes
+// p.block_n set by the caller; CLUSTER = 2 is the SM-pair form (256-row tiles, multicast B halves)
+template <int EPI, int CONVW, int CLUSTER>
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream, int split_k = 1,
+                       void* ws = nullptr, long long ws_bytes = 0) {
+  // MMA width: the 1-CTA kernel runs 128- and 256-wide tiles only
+  const int nm = p.block_n == 256 ? 2 : p.block_n == 128 ? 1 : 0;
+  if (CLUSTER == 1 && nm == 0) return YB_ERR_ARG;
+  auto kern = nm == 2 ? gemm_kernel<EPI, CONVW, CLUSTER, 256> : nm == 1 ? gemm_kernel<EPI, CONVW, CLUSTER, 128>
+                      : gemm_kernel<EPI, CONVW, CLUSTER, CLUSTER == 1 ? 128 : 64>;
+  static bool attr_set[3][kMaxDevices] = {};
+  if (int rc = ensure_dynamic_smem(kern, GEMM_SMEM_BYTES, attr_set[nm], "gemm")) return rc;
+  if (CLUSTER == 2) p.num_m_tiles = p.conv ? (p.num_m_tiles + 1) / 2 : (p.M + 255) / 256;   // conv: pairs of 128-voxel boxes
+  else if (!p.conv) p.num_m_tiles = (p.M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   p.num_n_tiles = (p.N + p.block_n - 1) / p.block_n;
-  int stages = (227 * 1024 - 256 - PAIR_EPI_STAGE_BYTES - 1024) / pair_stage_bytes(p.block_n);
-  p.stages = stages > PAIR_MAX_STAGES ? PAIR_MAX_STAGES : stages;
+  p.stages = gemm_stages(p.block_n, CONVW);
   const int tiles = p.num_m_tiles * p.num_n_tiles;
-  // persistent grid = the number of CTA pairs the device can hold at once (GPCs with an odd SM count leave an SM unpaired;
-  // asked of the driver once per device, the SM count / 2 if the query is unavailable)
+  // persistent grid: one CTA per SM, or the number of CTA pairs the device holds at once (asked of the driver once per device)
   static int max_clusters[kMaxDevices] = {0};
   const int dev = current_device();
-  if (max_clusters[dev] == 0) max_clusters[dev] = pair_max_clusters(kern);
+  if (max_clusters[dev] == 0) max_clusters[dev] = CLUSTER == 2 ? pair_max_clusters(kern) : sm_count();
   p.sk_full = tiles; p.sk_ns = 1; p.sk_per = 0; p.sk_ws = nullptr;
   int tail = 0;
-  if (EPI == YB_EPI_GATE_RES && !p.conv && ws != nullptr && split_k != 1) {
+  if (CLUSTER == 2 && EPI == YB_EPI_GATE_RES && !p.conv && ws != nullptr && split_k != 1) {
     const int num_kb = (p.K + GEMM_BLOCK_K - 1) / GEMM_BLOCK_K;
     gemm_splitk_plan(tiles, num_kb, max_clusters[dev], split_k, &p.sk_full, &p.sk_ns, &p.sk_per);
     tail = tiles - p.sk_full;
@@ -917,27 +679,25 @@ static int launch_gemm_pair(const CUtensorMap& tmA, const CUtensorMap& tmB, Gemm
     if (tail > 0) p.sk_ws = static_cast<float*>(ws);
   }
   const int work = p.sk_full + tail * p.sk_ns;
-  const int clusters = work < max_clusters[dev] ? work : max_clusters[dev];
-  kern<<<2 * clusters, GEMM_THREADS, pair_smem_bytes(p.block_n, p.stages), stream>>>(tmA, tmB, p);
-  int rc = check_launch("gemm_pair");
+  const int groups = work < max_clusters[dev] ? work : max_clusters[dev];
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(groups * CLUSTER);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = GEMM_SMEM_BYTES;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = CLUSTER;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = 1;
+  cfg.attrs = &attr;
+  cfg.numAttrs = 1;
+  (void)cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p);   // a failed launch is reported by check_launch
+  int rc = check_launch("gemm");
   if (rc || tail == 0) return rc;
   const long long total = static_cast<long long>(tail) * 256 * (p.block_n / 4);
   gemm_splitk_combine_kernel<<<static_cast<int>((total + 255) / 256), 256, 0, stream>>>(p, tail);
   return check_launch("gemm_splitk_combine");
-}
-
-template <int BLOCK_N, int EPI, int CONVW = 0>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BLOCK_N, CONVW>;
-  auto kern = gemm_kernel<BLOCK_N, EPI, CONVW>;
-  static bool attr_set[kMaxDevices] = {false};
-  if (int rc = ensure_dynamic_smem(kern, Cfg::SMEM_BYTES, attr_set, "gemm")) return rc;
-  if (!p.conv) p.num_m_tiles = (p.M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
-  p.num_n_tiles = (p.N + BLOCK_N - 1) / BLOCK_N;
-  const int tiles = p.num_m_tiles * p.num_n_tiles;
-  const int grid = tiles < sm_count() ? tiles : sm_count();
-  kern<<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  return check_launch("gemm");
 }
 
 // Tile plan of one conv launch (pure host arithmetic; exported as yb_conv3d_plan for the CPU test-suite).
@@ -997,15 +757,17 @@ extern "C" int yb_gemm_sp_qkv(const void* A, long long lda, const void* W, const
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmB, W, p.N, K, K, p.block_n / 2, GEMM_BLOCK_K);
   if (rc) return rc;
-  return launch_gemm_pair<YB_EPI_SP_QKV>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream_));
+  return launch_gemm<YB_EPI_SP_QKV, 0, 2>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream_));
 }
 
+// Automatic kernel / tile choice of yb_gemm_bf16: the 1-CTA kernel for every shape. On the H100 (700 W) the SM-pair form measured
+// 321-339 TFLOP/s on the three DiT GEMM shapes at L = 18 480 against 624-684 for the 1-CTA kernel, so it runs only when asked for
+// (cta_pair = 2) and as the fused Ulysses q|k|v all-to-all (yb_gemm_sp_qkv).
 extern "C" int yb_gemm_plan(int M, int N, int sms, int* out4) {
   if (M <= 0 || N <= 0 || sms < 2 || !out4) return YB_ERR_ARG;
-  const bool pair = M >= 1024 && N >= 128;
-  out4[0] = pair ? 1 : 0;
-  out4[1] = pair ? yb::pair_block_n(M, N, sms / 2) : ((N % 256 == 0 || N > 1024) ? 256 : 128);
-  out4[2] = pair ? (M + 255) / 256 : (M + 127) / 128;
+  out4[0] = 0;
+  out4[1] = (N % 256 == 0 || N > 1024) ? 256 : 128;
+  out4[2] = (M + yb::GEMM_BLOCK_M - 1) / yb::GEMM_BLOCK_M;
   out4[3] = (N + out4[1] - 1) / out4[1];
   return YB_OK;
 }
@@ -1031,13 +793,13 @@ extern "C" int yb_gemm_splitk_plan(int tiles, int num_kb, int clusters, int spli
 extern "C" long long yb_gemm_workspace_bytes(int M, int N, int K, int epilogue, int cta_pair, int split_k) {
   using namespace yb;
   if (M <= 0 || N <= 0 || K <= 0 || epilogue != YB_EPI_GATE_RES || split_k == 1 || split_k < 0 || split_k > 12) return 0;
-  if (!(cta_pair == 2 || (cta_pair == 0 && M >= 1024 && N >= 128))) return 0;
+  if (cta_pair != 2) return 0;   // only the SM-pair kernel splits
   static int max_clusters[kMaxDevices] = {0};
   static bool attr_set[kMaxDevices] = {false};
   const int dev = current_device();
   if (max_clusters[dev] == 0) {   // same query, same kernel attributes as the launch path: the two plans must agree
-    if (ensure_dynamic_smem(gemm_pair_kernel<YB_EPI_GATE_RES>, 227 * 1024, attr_set, "gemm_pair")) return 0;
-    max_clusters[dev] = pair_max_clusters(gemm_pair_kernel<YB_EPI_GATE_RES>);
+    if (ensure_dynamic_smem(gemm_kernel<YB_EPI_GATE_RES, 0, 2, 256>, GEMM_SMEM_BYTES, attr_set, "gemm")) return 0;
+    max_clusters[dev] = pair_max_clusters(gemm_kernel<YB_EPI_GATE_RES, 0, 2, 256>);
   }
   const int bn = pair_block_n(M, N, max_clusters[dev]);
   const int tiles = ((M + 255) / 256) * ((N + bn - 1) / bn);
@@ -1088,9 +850,8 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
   int rc = make_tmap_bf16_3d(&tmA, a->A, a_chunks, a->M, a_split, a->lda, a_chunks > 1 ? a_chunk_ld : a->lda * (long long)a->M + 8,
                              GEMM_BLOCK_M, GEMM_BLOCK_K);
   if (rc) return rc;
-  // SM-pair kernel for the large token GEMMs (auto: M >= 1024 rows and N >= 128); the 1-CTA kernel keeps the small ones
-  // (context / embedding projections: a 256-row tile pair would be mostly padding) and every conv mode
-  const bool pair = a->cta_pair == 2 || (a->cta_pair == 0 && a->M >= 1024 && a->N >= 128);
+  // SM-pair kernel only when asked for (see yb_gemm_plan)
+  const bool pair = a->cta_pair == 2;
   if (pair) {
     int bn = a->block_n;
     if (bn == 0) bn = pair_block_n(a->M, a->N, sm_count() / 2);
@@ -1099,32 +860,26 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
     rc = make_tmap_bf16_2d(&tmB, a->B, a->N, a->K, a->ldb, bn / 2, GEMM_BLOCK_K);
     if (rc) return rc;
     switch (a->epilogue) {
-      case YB_EPI_BF16: return launch_gemm_pair<YB_EPI_BF16>(tmA, tmB, p, stream);
-      case YB_EPI_GELU_BF16: return launch_gemm_pair<YB_EPI_GELU_BF16>(tmA, tmB, p, stream);
-      case YB_EPI_F32: return launch_gemm_pair<YB_EPI_F32>(tmA, tmB, p, stream);
-      case YB_EPI_GELU_ERF_BF16: return launch_gemm_pair<YB_EPI_GELU_ERF_BF16>(tmA, tmB, p, stream);
-      case YB_EPI_RES_BF16: return launch_gemm_pair<YB_EPI_RES_BF16>(tmA, tmB, p, stream);
-      default: return launch_gemm_pair<YB_EPI_GATE_RES>(tmA, tmB, p, stream, a->split_k, a->ws, a->ws_bytes);
+      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmB, p, stream);
+      case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 2>(tmA, tmB, p, stream);
+      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmB, p, stream);
+      case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 2>(tmA, tmB, p, stream);
+      case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmB, p, stream);
+      default: return launch_gemm<YB_EPI_GATE_RES, 0, 2>(tmA, tmB, p, stream, a->split_k, a->ws, a->ws_bytes);
     }
   }
   const int block_n = (a->block_n == 128 || a->block_n == 256) ? a->block_n : ((a->N % 256 == 0 || a->N > 1024) ? 256 : 128);
   rc = make_tmap_bf16_2d(&tmB, a->B, a->N, a->K, a->ldb, block_n, GEMM_BLOCK_K);
   if (rc) return rc;
-#define YB_DISPATCH(BN)                                                                  \
-  switch (a->epilogue) {                                                                 \
-    case YB_EPI_BF16: return launch_gemm<BN, YB_EPI_BF16>(tmA, tmB, p, stream);           \
-    case YB_EPI_GELU_BF16: return launch_gemm<BN, YB_EPI_GELU_BF16>(tmA, tmB, p, stream); \
-    case YB_EPI_F32: return launch_gemm<BN, YB_EPI_F32>(tmA, tmB, p, stream);             \
-    case YB_EPI_GELU_ERF_BF16: return launch_gemm<BN, YB_EPI_GELU_ERF_BF16>(tmA, tmB, p, stream); \
-    case YB_EPI_RES_BF16: return launch_gemm<BN, YB_EPI_RES_BF16>(tmA, tmB, p, stream);   \
-    default: return launch_gemm<BN, YB_EPI_GATE_RES>(tmA, tmB, p, stream);                \
+  p.block_n = block_n;
+  switch (a->epilogue) {
+    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 1>(tmA, tmB, p, stream);
+    case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 1>(tmA, tmB, p, stream);
+    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 1>(tmA, tmB, p, stream);
+    case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 1>(tmA, tmB, p, stream);
+    case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 1>(tmA, tmB, p, stream);
+    default: return launch_gemm<YB_EPI_GATE_RES, 0, 1>(tmA, tmB, p, stream);
   }
-  if (block_n == 256) {
-    YB_DISPATCH(256)
-  } else {
-    YB_DISPATCH(128)
-  }
-#undef YB_DISPATCH
 }
 
 
@@ -1155,10 +910,8 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
   if (st_t > 1) oT = (a->T - kt) / st_t + 1;
   if (st_hw > 1) { oH = (a->H + 1 - kh) / st_hw + 1; oW = (a->W + 1 - kw) / st_hw + 1; }
   if (oT <= 0 || oH <= 0 || oW <= 0) return YB_ERR_SHAPE;
-  // SM-pair kernel: 1 = forced, 2 = forced off, 0 = automatic — taken for output widths the 1-CTA kernel has to cut into a 128-wide
-  // tile plus a padded remainder (192, 384 channels of the Wan2.1 decoder: 1006 vs 678 and 832 vs 787 TFLOP/s measured); the other
-  // widths keep the 1-CTA kernel, whose kw-fused mode (3x less A traffic) wins there (profiles/r02_gemm_pair.md)
-  const bool conv_pair = a->cta_pair == 1 || (a->cta_pair == 0 && a->fuse_w != 2 && a->Cout > 128 && a->Cout % 256 != 0 && a->Cout <= 512);
+  // SM-pair kernel: 1 = forced; 0 (automatic) and 2 run the 1-CTA kernel, the faster of the two on the H100 (see yb_gemm_plan)
+  const bool conv_pair = a->cta_pair == 1;
   conv_plan(oT, oH, oW, block_n, kw, (conv_pair || strided) ? 1 : a->fuse_w, &p.TW, &p.TH, &p.TT, &fuse_w);
   p.tiles_w = (oW + p.TW - 1) / p.TW;
   p.tiles_h = (oH + p.TH - 1) / p.TH;
@@ -1193,8 +946,7 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
   rc = make_tmap_bf16_2d(&tmB, a->w, a->Cout, static_cast<uint64_t>(taps) * a->Cp, static_cast<uint64_t>(taps) * a->Cp,
                          block_n, GEMM_BLOCK_K);
   if (rc) return rc;
-  // SM-pair kernel (un-fused taps; each CTA of the pair owns one 128-voxel box, the weight tile is split between them):
-  // selected by a->cta_pair (1 = always, 0 = never until the per-width crossover is measured; see DESIGN.md §7)
+  // SM-pair kernel (un-fused taps; each CTA of the pair owns one 128-voxel box, the weight tile is split between them)
   if (conv_pair && !fuse_w) {
     p.conv = 1;
     p.block_n = a->Cout <= 256 ? a->Cout : (a->Cout % 192 == 0 ? 192 : 256);
@@ -1203,25 +955,22 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
                            p.block_n / 2, GEMM_BLOCK_K);
     if (rc) return rc;
     switch (a->epilogue) {
-      case YB_EPI_BF16: return launch_gemm_pair<YB_EPI_BF16>(tmA, tmBp, p, stream);
-      case YB_EPI_F32: return launch_gemm_pair<YB_EPI_F32>(tmA, tmBp, p, stream);
-      default: return launch_gemm_pair<YB_EPI_RES_BF16>(tmA, tmBp, p, stream);
+      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmBp, p, stream);
+      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmBp, p, stream);
+      default: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmBp, p, stream);
     }
   }
-#define YB_CONV_DISPATCH(BN, CW)                                                              \
+  p.block_n = block_n;
+#define YB_CONV_DISPATCH(CW)                                                                  \
   switch (a->epilogue) {                                                                     \
-    case YB_EPI_BF16: return launch_gemm<BN, YB_EPI_BF16, CW>(tmA, tmB, p, stream);           \
-    case YB_EPI_F32: return launch_gemm<BN, YB_EPI_F32, CW>(tmA, tmB, p, stream);             \
-    default: return launch_gemm<BN, YB_EPI_RES_BF16, CW>(tmA, tmB, p, stream);                \
+    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, CW, 1>(tmA, tmB, p, stream);            \
+    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, CW, 1>(tmA, tmB, p, stream);              \
+    default: return launch_gemm<YB_EPI_RES_BF16, CW, 1>(tmA, tmB, p, stream);                 \
   }
-  if (block_n == 256 && fuse_w) {
-    YB_CONV_DISPATCH(256, 1)
-  } else if (block_n == 256) {
-    YB_CONV_DISPATCH(256, 0)
-  } else if (fuse_w) {
-    YB_CONV_DISPATCH(128, 1)
+  if (fuse_w) {
+    YB_CONV_DISPATCH(1)
   } else {
-    YB_CONV_DISPATCH(128, 0)
+    YB_CONV_DISPATCH(0)
   }
 #undef YB_CONV_DISPATCH
 }

@@ -536,7 +536,7 @@ __global__ void unpatchify2_clamp_kernel(const float* __restrict__ y, long long 
 
 inline int grid_for(long long total) {
   long long b = (total + 255) / 256;
-  const long long cap = 148LL * 16;
+  const long long cap = static_cast<long long>(sm_count()) * 16;
   return static_cast<int>(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
@@ -550,7 +550,7 @@ extern "C" int yb_gn_stats(const void* x, long long ld, void* stats, long long N
   if ((ld % 8) || (reinterpret_cast<uintptr_t>(x) & 0xF)) return YB_ERR_ALIGNMENT;
   const int vox_per_block = 256 / (C / 8);
   long long blocks = (N + vox_per_block - 1) / vox_per_block;
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > sm_count() * 8) blocks = sm_count() * 8;
   gn_stats_kernel<<<static_cast<int>(blocks), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const __nv_bfloat16*>(x), ld, static_cast<double*>(stats), N, C, G);
   return check_launch("gn_stats");
@@ -655,7 +655,7 @@ extern "C" int yb_vae_rms_act(const void* x, long long ldx, void* out, const voi
   const int g = nch > 1 ? 32 : (Cp <= 64 ? 8 : (Cp <= 128 ? 16 : 32));         // lanes per voxel
   const int per_block = 8 * (4 / nch) * (32 / g);
   long long blocks = (nvox + per_block - 1) / per_block;
-  if (blocks > 148LL * 32) blocks = 148LL * 32;
+  if (blocks > static_cast<long long>(sm_count()) * 32) blocks = static_cast<long long>(sm_count()) * 32;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
 #define YB_RMS_LAUNCH(NCH, G)                                                                                        \
   rms_act_kernel<NCH, G><<<static_cast<int>(blocks), 256, 0, st>>>(static_cast<const __nv_bfloat16*>(x), ldx,         \

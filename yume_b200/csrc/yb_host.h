@@ -104,7 +104,7 @@ inline int sm_count() {
   if (n[dev] == 0) {
     int v = 0;
     cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev);
-    n[dev] = v > 0 ? v : 148;
+    n[dev] = v > 0 ? v : 132;   // H100 SXM
   }
   return n[dev];
 }

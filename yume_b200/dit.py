@@ -1,4 +1,4 @@
-"""WanDiT — the B200 denoise-forward engine behind the reference's `WanModel.forward`.
+"""WanDiT — the H100 denoise-forward engine behind the reference's `WanModel.forward`.
 
 One engine instance owns the re-packed weights of one WanModel (5B `wan23` tree or 14B `wan` tree) and runs the
 whole forward through libyume_b200.so. Host code here is orchestration only: shapes, the FramePack segment plan,
@@ -121,7 +121,7 @@ def sp_shard(L: int, world: int, rank: int) -> Tuple[int, int, int]:
 
 
 class WanDiT:
-    """B200 engine for one WanModel. `variant` is '5b' (wan23 tree) or '14b' (wan tree)."""
+    """H100 engine for one WanModel. `variant` is '5b' (wan23 tree) or '14b' (wan tree)."""
 
     def __init__(self, state_dict: Dict[str, Tensor], variant: str, dim: int, ffn_dim: int, num_heads: int,
                  num_layers: int, in_dim: int, out_dim: int, text_len: int = 512, freq_dim: int = 256,

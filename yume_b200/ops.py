@@ -62,7 +62,7 @@ def gemm(a: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: to
          n_split: int = 0, split_stride: int = 0, a_split: int = 0, a_split_stride: int = 0,
          shape: Optional[tuple] = None, res: Optional[torch.Tensor] = None, cta_pair: int = 0, split_k: Optional[int] = None) -> torch.Tensor:
     """out = epi(a[M,K] @ w[N,K]^T + bias). a, w bf16 (2-D, row stride arbitrary); see include/yume_b200.h.
-    cta_pair: 0 automatic, 1 force the 1-CTA kernel, 2 force the SM-pair (cta_group::2) kernel.
+    cta_pair: 0 automatic, 1 force the 1-CTA kernel, 2 force the SM-pair kernel (2-CTA cluster, multicast B operand).
     split_k (SM-pair GATE_RES launches): 0 automatic tail split-K, 1 never, 2..12 force that many K segments on the last wave."""
     global _launches, _flops
     _need(a, torch.bfloat16, "a")
@@ -209,7 +209,7 @@ def attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tens
               split: int = 0) -> torch.Tensor:
     """softmax(q k^T * scale) v, non-causal. q [Lq, heads*128], k/v [Lk, heads*128] bf16 (row strides arbitrary).
     split: KV split policy (YB_ATT_SPLIT_SHIFT): 0 automatic tail split, 1 never, 2..4 force that many KV segments.
-    variant: 0 product kernel (P in TMEM), 1 debug (P through smem)."""
+    variant: 0 product kernel (P in registers), 1 debug (P through smem)."""
     global _launches, _flops
     for n, t in (("q", q), ("k", k), ("v", v), ("out", out)):
         _need(t, torch.bfloat16, n)
@@ -310,7 +310,7 @@ def linear_f32(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], o
 
 
 def umma_probe(a: torch.Tensor, b: torch.Tensor, mode: int) -> torch.Tensor:
-    """tcgen05 self-test (tests only). a, b bf16 [128,128] contiguous -> f32 [128,128]."""
+    """wgmma / TMA self-test (tests only). a, b bf16 [128,128] contiguous -> f32 [128,128]."""
     _need(a, torch.bfloat16, "a")
     _need(b, torch.bfloat16, "b")
     d = torch.empty(128, 128, device=a.device, dtype=torch.float32)
@@ -324,8 +324,7 @@ def umma_probe(a: torch.Tensor, b: torch.Tensor, mode: int) -> torch.Tensor:
 YB_EPI_RES_BF16 = YB_EPI_RES_BF16
 
 
-# kernel choice of conv3d_causal when the caller does not say (0 = 1-CTA kernel, 1 = SM-pair kernel); set per engine after the
-# per-width crossover measurement (profiles/README.md)
+# kernel choice of conv3d_causal when the caller does not say (see yb_conv3d_args.cta_pair in include/yume_b200.h)
 CONV_CTA_PAIR = 0
 GEMM_SPLIT_K = 0     # tail split-K policy of the SM-pair gate+residual GEMM for callers that do not pass one: 0 automatic, 1 never
 

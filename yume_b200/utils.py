@@ -48,7 +48,7 @@ class KernelTimer:
 class ClockSampler:
     """Samples SM clocks and throttle reasons of one GPU in a background thread while a timed region runs: NVML every 20 ms
     when `pynvml` can open the device (a 40 ms multi-GPU step still gets several samples under load), else the `nvidia-smi`
-    query line of /opt/skills/guides/B200_PROFILING.md every 200 ms. Both read the same driver counters."""
+    query line below every 200 ms. Both read the same driver counters."""
 
     QUERY = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
              "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"

@@ -1,4 +1,4 @@
-"""B200 decode path of the HunyuanVideo causal 3D VAE (`AutoencoderKLCausal3D.decode`, SURVEY.md §8 rows a17-a19).
+"""H100 decode path of the HunyuanVideo causal 3D VAE (`AutoencoderKLCausal3D.decode`, SURVEY.md §8 rows a17-a19).
 
 Reference (file:line in /root/reference/hyvideo/vae):
   autoencoder_kl_causal_3d.py:297-341 decode/_decode, :343-359 blend_v/h/t, :417-463 spatial tiling, :500-531 temporal
@@ -10,8 +10,8 @@ Layer table per tile z [16, T, H, W] (upstream 884-16c config, SURVEY.md Appendi
   up0: 3 resnets @512, up (1,2,2)+conv | up1: 3 resnets @512, up (2,2,2)+conv | up2: 3 resnets 512->256, up (2,2,2)+conv |
   up3: 3 resnets 256->128 | GroupNorm, SiLU, conv_out 128->3
 
-B200 mapping: activations are channels-last bf16 [T*H*W, C]. Every 3x3x3 CausalConv3d is an implicit GEMM on the
-tcgen05 kernel (yb_conv3d_causal: 4-D TMA boxes over a replicate-padded buffer, no im2col); GroupNorm-apply + SiLU +
+H100 mapping: activations are channels-last bf16 [T*H*W, C]. Every 3x3x3 CausalConv3d is an implicit GEMM on the
+wgmma kernel (yb_conv3d_causal: 4-D TMA boxes over a replicate-padded buffer, no im2col); GroupNorm-apply + SiLU +
 nearest upsample + replicate padding are ONE gather pass that writes that padded buffer (yb_vae_pad_act); the resnet
 skip add rides in the conv epilogue (YB_EPI_RES_BF16); the mid-block attention is five GEMM calls around a
 frame-causal softmax kernel (no [L, L] mask tensor is ever built; the reference builds it with a Python loop over L).

@@ -1,10 +1,10 @@
-"""B200 decode path of the Wan2.1 VAE (`WanVAE.decode`) — the VAE the 14B sampler calls (wan/image2video.py:197,
+"""H100 decode path of the Wan2.1 VAE (`WanVAE.decode`) — the VAE the 14B sampler calls (wan/image2video.py:197,
 fastvideo/sample/sample.py). SURVEY.md §8(f) "next" row, rank 1 (second half).
 
 Reference: /root/reference/wan/modules/vae.py (≡ wan23/modules/vae2_1.py) — `WanVAE_.decode` (:544-568) decodes one
 latent frame per `Decoder3d.forward` call through a per-conv feature cache. As for the 2.2 VAE (yume_b200/vae22.py, whose
-building blocks this engine reuses) the cache logic unrolls to causal convs over the whole sequence, so the B200 path is a
-single pass of tcgen05 implicit-GEMM convs with TMA zero fill as the padding. What differs from 2.2: the flat
+building blocks this engine reuses) the cache logic unrolls to causal convs over the whole sequence, so the H100 path is a
+single pass of wgmma implicit-GEMM convs with TMA zero fill as the padding. What differs from 2.2: the flat
 `decoder.upsamples` Sequential (:395-414), `Resample`'s Conv2d halves the channels (:76-83) so blocks 1..3 start at
 dims[i] // 2 (:398-399), there is no DupUp3D shortcut, and the head conv emits RGB directly (no unpatchify).
 """

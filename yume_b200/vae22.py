@@ -1,15 +1,16 @@
-"""B200 decode path of the Wan2.2 VAE (`Wan2_2_VAE.decode`) — the VAE the Yume-5B sampler actually calls
+"""H100 decode path of the Wan2.2 VAE (`Wan2_2_VAE.decode`) — the VAE the Yume-5B sampler actually calls
 (wan23/textimage2video.py:124; fastvideo/sample/sample_5b.py:1051-1052). SURVEY.md §8(f) "next" row, rank 1.
 
 Reference: /root/reference/wan23/modules/vae2_2.py — `WanVAE_.decode` (:831-860) feeds ONE latent frame at a time through
 `Decoder3d` and threads a feature cache through every `CausalConv3d` (:34-44, :216-239, :114-170, :681-737); a Python
 loop of T iterations, each launching the whole decoder on a single frame.
 
-B200 redesign: unrolling the cache logic shows every conv is a causal convolution over the whole frame sequence with
+H100 redesign: unrolling the cache logic shows every conv is a causal convolution over the whole frame sequence with
 zero padding in front (frame 0 skips `time_conv`, `time_conv` never sees frame 0, `DupUp3D` drops its first
-factor_t-1 frames — oracle/wan22vae.py states this and is pinned to the reference's chunked output). With 180 GB of
-HBM the whole sequence fits, so the decode is ONE pass over [T, H, W, C] channels-last bf16 tensors:
-  * every conv (3x3x3, Conv2d 3x3 = (1,3,3), time_conv = (3,1,1)) is the tcgen05 implicit GEMM `yb_conv3d_causal` with
+factor_t-1 frames — oracle/wan22vae.py states this and is pinned to the reference's chunked output). The decode is
+therefore ONE pass over [T, H, W, C] channels-last bf16 tensors; the whole sequence must fit in device memory (on an 80 GB H100
+a 49-frame 704x1280 chunk does, the 81-frame video does not):
+  * every conv (3x3x3, Conv2d 3x3 = (1,3,3), time_conv = (3,1,1)) is the wgmma implicit GEMM `yb_conv3d_causal` with
     `oob_zero_pad`: the causal zero padding is TMA out-of-bounds fill on the UNPADDED activation — no padded copy, no
     feature cache, no per-frame launches;
   * RMS_norm + SiLU (+ nearest-exact 2x upsample) is one gather pass (`yb_vae_rms_act`);

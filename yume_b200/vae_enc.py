@@ -1,12 +1,12 @@
-"""B200 ENCODE paths of the two Wan VAEs — SURVEY.md §8(f) "next" row, rank 3: the conditioning / history encodes the samplers
+"""H100 ENCODE paths of the two Wan VAEs — SURVEY.md §8(f) "next" row, rank 3: the conditioning / history encodes the samplers
 run before the denoise loop (`Wan2_2_VAE.encode`, fastvideo/sample/sample_5b.py:892-893; `WanVAE.encode`,
 wan/image2video.py:348-367).
 
 Reference: /root/reference/wan23/modules/vae2_2.py `WanVAE_.encode` (:796-829) and /root/reference/wan/modules/vae.py (:515-542)
 encode frame 0 alone and then 4 frames per `Encoder3d.forward` call, threading a feature cache through every `CausalConv3d`.
 Unrolled (oracle/wan22vae_enc.py, oracle/wan21vae_enc.py, both pinned to the reference's chunked output) every conv is a causal
-conv over the whole frame sequence, so the B200 path is the decoder's design run backwards: ONE pass over channels-last bf16
-[T, H, W, C] tensors on the tcgen05 implicit-GEMM conv, with the two strided `Resample` convs done by the tensor map itself —
+conv over the whole frame sequence, so the H100 path is the decoder's design run backwards: ONE pass over channels-last bf16
+[T, H, W, C] tensors on the wgmma implicit-GEMM conv, with the two strided `Resample` convs done by the tensor map itself —
   * `Resample(downsample2d)`: ZeroPad2d((0,1,0,1)) + Conv2d(3x3, stride 2) (vae2_2.py:101-104) = `yb_conv3d_causal` with
     `stride_hw = 2`: TMA `elementStrides` sample every second voxel, the pad row/column behind the data is out-of-bounds fill;
   * `Resample(downsample3d)` (:105-110, :158-170): frame 0 bypasses `time_conv`, the rest is CausalConv3d((3,1,1),
