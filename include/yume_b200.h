@@ -287,7 +287,10 @@ int yb_blend(const void* a, void* b, long long outer, int ea, int eb, int ext, l
 /* One-pass assembly of a tiled decode (temporal_tiled_decode / spatial_tiled_decode + blend_v / blend_h / blend_t,
  * autoencoder_kl_causal_3d.py:343-359, 417-463, 500-531): the final f32 [C, F, H, W] video straight from the RAW decoded tiles — each
  * output voxel is the reference's in-place cross-fade sequence written out as one expression of <= 2 x 4 raw tile values (same
- * operations, same order), so tiles may be decoded in any order / on any GPU and no torch.cat or per-row blend launch remains.
+ * operations, same order, bit for bit: weights rounded from double, products and sums rounded separately as torch does), so tiles
+ * may be decoded in any order / on any GPU and no torch.cat or per-row blend launch remains. Exact when no tile is read back inside
+ * its own blended region: every interior tile k of a row / column / window sequence has size >= ext(k) + ext(k+1), ext(k) = the
+ * clamped blend extent with its predecessor (tile overlap factors <= 0.5 always satisfy this).
  *   tile_ptrs  DEVICE array [nt*ni*nj] of device pointers: tile (ti, i, j) = f32 [C, tlen[ti] + tskip(ti), th[i], tw[j]] contiguous,
  *              tskip(ti) = 1 for ti > 0 (the first decoded frame of later temporal tiles is dropped, :519-520), else 0
  *   th, tw, tlen, tf0   DEVICE int arrays: tile heights [ni] / widths [nj] in pixels, kept-length source frames [nt] (after the

@@ -222,7 +222,10 @@ __global__ void blend_kernel(const float* __restrict__ a, float* __restrict__ b,
 // with its upper / left / previous neighbour (blend_v, blend_h, blend_t, :343-359), crops and torch.cat's rows, then columns, then
 // time. Every output voxel is therefore a fixed expression of at most 2 (time) x 4 (space) RAW tile values; this kernel evaluates
 // that expression directly from the raw tiles into the final [C, F, H, W] video — same operations, same order, same fp32
-// roundings as the in-place sequence (a*(1-w) + b*w per blend) — so tiles can be decoded in any order, on any GPU.
+// roundings as the in-place sequence (xfade below), bit for bit — so tiles can be decoded in any order, on any GPU.
+// A neighbour enters with its own blends applied only where they touch the rows / columns / frames read from it, which holds
+// when no tile is read back inside its own blended region: size(k) >= ext(k) + ext(k+1) for every interior tile k
+// (ops.vae_assemble_tiles checks it; tile overlap factors <= 0.5 always satisfy it).
 //   tiles   table of raw decoded tiles: tile (ti, i, j) is f32 [C, ft, h_i, w_j] contiguous at ptr[(ti*ni + i)*nj + j]
 //   space   tile (i, j) covers output rows [i*rl, i*rl + min(rl, h_i)), blended over its first ev rows with tile (i-1, j):
 //           ev = min(h_{i-1}, h_i, E) (blend_v clamps the extent to both tiles); columns likewise
@@ -245,6 +248,12 @@ __device__ __forceinline__ float tile_at(const TileAsm& a, int ti, int i, int j,
   const int skip = ti > 0 ? 1 : 0;   // later temporal tiles: the first decoded frame is dropped (dec[:, :, 1:], :519-520)
   return t[((static_cast<long long>(c) * (a.tlen[ti] + skip) + f + skip) * a.th[i] + y) * a.tw[j] + x];
 }
+// One cross-fade step of blend_v / blend_h / blend_t: `a * (1 - y / ext) + b * (y / ext)` on f32 tensors. Python computes both
+// weights in double and torch rounds them to f32; each product and the sum is rounded on its own (no fused multiply-add).
+__device__ __forceinline__ float xfade(float a, float b, int y, int ext) {
+  const double r = static_cast<double>(y) / static_cast<double>(ext);
+  return __fadd_rn(__fmul_rn(a, static_cast<float>(1.0 - r)), __fmul_rn(b, static_cast<float>(r)));
+}
 // fully blended value of spatial tile (i, j) of temporal tile ti at (y, x): blend_v with the upper neighbour first, then blend_h
 // with the left neighbour (the reference's order, :440-448); neighbours enter with THEIR blends applied, which for the rows /
 // columns read here (their last `ext` ones) reduces to one more blend with raw tiles
@@ -252,27 +261,18 @@ __device__ __forceinline__ float spatial_value(const TileAsm& a, int ti, int i, 
   const int ev = i > 0 ? min(min(a.th[i - 1], a.th[i]), a.E) : 0;
   const int eh = j > 0 ? min(min(a.tw[j - 1], a.tw[j]), a.E) : 0;
   const bool bv = y < ev, bh = x < eh;
-  const float wv = bv ? static_cast<float>(y) / static_cast<float>(ev) : 1.f;
-  const float wh = bh ? static_cast<float>(x) / static_cast<float>(eh) : 1.f;
   float v = tile_at(a, ti, i, j, c, f, y, x);
   if (bv) {   // upper tile's row (already blended horizontally with ITS left neighbour on these columns)
     const int r = a.th[i - 1] - ev + y;
     float u = tile_at(a, ti, i - 1, j, c, f, r, x);
-    if (bh) {
-      const int eh_u = min(min(a.tw[j - 1], a.tw[j]), a.E);   // same column pair
-      const float ul = tile_at(a, ti, i - 1, j - 1, c, f, r, a.tw[j - 1] - eh_u + x);
-      u = ul * (1.f - wh) + u * wh;
-    }
-    v = u * (1.f - wv) + v * wv;
+    if (bh) u = xfade(tile_at(a, ti, i - 1, j - 1, c, f, r, a.tw[j - 1] - eh + x), u, x, eh);
+    v = xfade(u, v, y, ev);
   }
   if (bh) {   // left tile's column (already blended vertically with ITS upper neighbour on these rows)
     const int cx = a.tw[j - 1] - eh + x;
     float lft = tile_at(a, ti, i, j - 1, c, f, y, cx);
-    if (bv) {
-      const float lu = tile_at(a, ti, i - 1, j - 1, c, f, a.th[i - 1] - ev + y, cx);
-      lft = lu * (1.f - wv) + lft * wv;
-    }
-    v = lft * (1.f - wh) + v * wh;
+    if (bv) lft = xfade(tile_at(a, ti, i - 1, j - 1, c, f, a.th[i - 1] - ev + y, cx), lft, y, ev);
+    v = xfade(lft, v, x, eh);
   }
   return v;
 }
@@ -296,11 +296,7 @@ __global__ void __launch_bounds__(256) vae_assemble_tiles_kernel(const TileAsm a
     float v = spatial_value(a, ti, i, j, c, f, y, x);
     if (ti > 0) {
       const int et = min(min(a.tlen[ti - 1], a.tlen[ti]), a.Et);
-      if (f < et) {
-        const float w = static_cast<float>(f) / static_cast<float>(et);
-        const float pv = spatial_value(a, ti - 1, i, j, c, a.tlen[ti - 1] - et + f, y, x);
-        v = pv * (1.f - w) + v * w;
-      }
+      if (f < et) v = xfade(spatial_value(a, ti - 1, i, j, c, a.tlen[ti - 1] - et + f, y, x), v, f, et);
     }
     out[idx] = v;
   }

@@ -440,6 +440,12 @@ def vae_assemble_tiles(tiles, th, tw, tlen, tf0, out: torch.Tensor, row_limit: i
     """tiles[ti][i][j]: raw decoded tiles f32 [C, frames, th[i], tw[j]] (contiguous); out f32 [C, F, H, W] (yb_vae_assemble_tiles)."""
     global _launches
     nt, ni, nj = len(tiles), len(tiles[0]), len(tiles[0][0])
+    for sizes, ext in ((th, blend_extent), (tw, blend_extent), (tlen, t_blend_extent)):
+        # the kernel reads a neighbour with only the blends that reach the rows it reads: no tile may be read back inside its
+        # own blended region (interior tile k: size >= ext(k) + ext(k+1)); tile overlaps <= 0.5 always satisfy this
+        cut = [min(sizes[k - 1], sizes[k], ext) for k in range(1, len(sizes))]
+        if any(sizes[k] < cut[k - 1] + cut[k] for k in range(1, len(sizes) - 1)):
+            raise YumeB200Error(f"vae_assemble_tiles: blend extent {ext} overlaps itself inside a tile of sizes {list(sizes)}")
     dev = out.device
     flat = [tiles[a][b][c] for a in range(nt) for b in range(ni) for c in range(nj)]
     for t in flat:
