@@ -254,7 +254,8 @@ int yb_linear_f32_small(const void* in, const void* W, const void* bias, void* o
                         void* stream);
 
 /* General fp32 linear (SIMT, exact fp32): out[M,N] = in[M,K] * W[N,K]^T + bias. Replaces Head.head
- * (wan23/modules/model.py:331,346) which the reference runs under autocast(fp32). N % 4 == 0, K % 4 == 0. */
+ * (wan23/modules/model.py:331,346) which the reference runs under autocast(fp32). N % 4 == 0, K % 4 == 0, ldi % 4 == 0
+ * (YB_ERR_SHAPE otherwise); in and W 16-byte aligned (YB_ERR_ALIGNMENT otherwise). */
 int yb_linear_f32(const void* in, long long ldi, const void* W, const void* bias, void* out, long long ldo, int M,
                   int N, int K, void* stream);
 
@@ -281,7 +282,9 @@ int yb_nhwc_to_nchw_f32(const void* x, long long ldx, void* out, long long N, in
  * `.float().clamp_(-1, 1)`) on the channels-last f32 head output. */
 int yb_nhwc_to_nchw_f32_clamp(const void* x, long long ldx, void* out, long long N, int Cn, float lo, float hi, void* stream);
 /* Tile cross-fade (blend_v / blend_h / blend_t, autoencoder_kl_causal_3d.py:343-359) on contiguous f32 tiles:
- * b[o, y, i] = a[o, ea-ext+y, i] * (1 - y/ext) + b[o, y, i] * (y/ext) for y < ext; a is [outer, ea, inner], b [outer, eb, inner]. */
+ * b[o, y, i] = a[o, ea-ext+y, i] * (1 - y/ext) + b[o, y, i] * (y/ext) for y < ext; a is [outer, ea, inner], b [outer, eb, inner].
+ * Bit-exact with the reference's expression on f32 tensors: the weights are computed in double and rounded to f32, and each
+ * product and the sum is rounded on its own (no fused multiply-add), as in yb_vae_assemble_tiles. */
 int yb_blend(const void* a, void* b, long long outer, int ea, int eb, int ext, long long inner, void* stream);
 
 /* One-pass assembly of a tiled decode (temporal_tiled_decode / spatial_tiled_decode + blend_v / blend_h / blend_t,

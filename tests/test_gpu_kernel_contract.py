@@ -766,3 +766,24 @@ def test_conv3d_causal_per_element(dev, T, H, W, ci, co, fuse_w, cta_pair):
     torch.cuda.synchronize()
     o32.check(tag + " F32")
     assert_within(o32.view, acc, Fb + 4 * U32 * acc.abs(), tag + " F32", "conv3d")
+
+
+# ------------------------------------------------------------------------------------------------------------
+# entry point -> tests that exercise it (tests/test_kernel_contract_cpu.py: every C-ABI entry point is in a COVERS table)
+# ------------------------------------------------------------------------------------------------------------
+COVERS = {
+    "yb_gemm_bf16": ["test_gemm_every_epilogue_per_element"],
+    "yb_attention_ex": ["test_attention_tails_scales_variants", "test_attention_production_heads",
+                        "test_attention_split_and_accumulate"],
+    "yb_ln_modulate": ["test_ln_modulate_every_instance"],
+    "yb_rmsnorm_rope_pieces": ["test_rmsnorm_rope_every_instance"],
+    "yb_qk_norm_rope": ["test_rmsnorm_rope_every_instance"],
+    "yb_sp_scatter_qkv": ["test_sp_scatter_qkv_on_one_gpu"],
+    "yb_attention_sp": ["test_attention_sp_on_one_gpu"],
+    "yb_vae_pad_act": ["test_vae_pad_act", "test_conv3d_causal_per_element"],
+    "yb_nhwc_to_nchw_f32": ["test_nhwc_to_nchw_f32"],
+    "yb_nhwc_to_nchw_f32_clamp": ["test_nhwc_to_nchw_f32"],
+    "yb_vae_assemble_tiles": ["test_vae_assemble_tiles_is_the_reference_blend_sequence"],
+    "yb_gn_stats": ["test_gn_stats_large_n_mean_much_larger_than_spread", "test_vae_pad_act"],
+    "yb_conv3d_causal": ["test_conv3d_causal_per_element"],
+}

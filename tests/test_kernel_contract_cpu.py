@@ -3,7 +3,12 @@
     overwritten, a 64-wide K block dropped from a GEMM tile, a 128-key tile dropped from an attention row), and accept the same
     results without the defect — computed here the way the kernels compute them (fp32 accumulation, bf16 P, bf16 output);
   * every template instance the .cu sources dispatch to (YB_LN_WARP, YB_RR_FAST, YB_RR_WARP, YB_QK_WARP, YB_SC) is in the GPU
-    file's width tables, with at least one width that reaches each general kernel — a new instance without a test fails here.
+    file's width tables, with at least one width that reaches each general kernel — a new instance without a test fails here;
+  * every C-ABI entry point of include/yume_b200.h is named in the COVERS table of one of the two GPU contract files (or is
+    exempt, with its reason), every test a table names exists, and a tested width reaches each YB_RMS_LAUNCH instance;
+  * the bounds of tests/test_gpu_kernel_contract_ext.py reject their defects (a next-frame key leaking into a masked softmax
+    row, an AvgDown group element dropped, replicate instead of zero padding on one conv face, a straddling n_split tile
+    sent to the wrong chunk, a token's sum of squares missing a head block) and accept the kernels' arithmetic.
 """
 import math
 import re
@@ -209,3 +214,189 @@ def test_coverage_guard_notices_a_width_removed_from_a_table(monkeypatch):
     monkeypatch.setattr(K, "RR_GENERAL_WIDTHS", (1024,))
     assert _coverage_problems(CSRC / "elementwise.cu") == ["YB_LN_WARP widths without a test: [5120]",
                                                           "no tested width reaches the general rmsnorm_rope kernel"]
+
+
+# ------------------------------------------------------------------------------------------------------------
+# C-ABI entry-point coverage guard
+# ------------------------------------------------------------------------------------------------------------
+import test_gpu_kernel_contract_ext as KX  # noqa: E402
+
+HEADER = Path(__file__).resolve().parents[1] / "include" / "yume_b200.h"
+EXEMPT = {
+    "yb_abi_version": "returns a constant; build() compares it with the Python side",
+    "yb_debug_force_split": "process-global test hook of the multi-GPU parity tool; sets a flag, launches nothing",
+    "yb_umma_probe": "self-test of the wgmma / TMA building blocks, not a product path (tests/test_gpu_parity.py)",
+}
+EXEMPT_SUFFIXES = {
+    "_plan": "host-only planner: no device code (pinned by the host-logic tests)",
+    "_workspace_bytes": "host-only workspace sizing: no device code",
+}
+
+
+def _entry_points(header):
+    return re.findall(r"^(?:int|long long)\s+(yb_\w+)\(", header.read_text(), flags=re.M)
+
+
+def _entry_problems(header, modules=(K, KX)):
+    problems, covered = [], set()
+    for mod in modules:
+        for entry, tests in mod.COVERS.items():
+            covered.add(entry)
+            for name in tests:
+                if not callable(getattr(mod, name, None)):
+                    problems.append(f"{mod.__name__}.COVERS[{entry!r}] names a test that does not exist: {name}")
+    entries = _entry_points(header)
+    if not entries:
+        problems.append("no entry points found in the header")
+    for entry in entries:
+        if entry in EXEMPT or any(entry.endswith(s) for s in EXEMPT_SUFFIXES):
+            continue
+        if entry not in covered:
+            problems.append(f"entry point without a contract test: {entry}")
+    return problems
+
+
+def test_every_entry_point_has_a_contract_test():
+    assert _entry_problems(HEADER) == []
+
+
+def test_entry_point_guard_notices_a_new_entry_point_and_a_missing_test(tmp_path, monkeypatch):
+    fake = tmp_path / "yume_b200.h"
+    fake.write_text(HEADER.read_text().replace("int yb_bcast_add(", "int yb_new_kernel(const void* x, void* stream);\n"
+                                               "int yb_bcast_add(", 1))
+    assert _entry_problems(fake) == ["entry point without a contract test: yb_new_kernel"]
+    covers = dict(KX.COVERS)
+    covers["yb_blend"] = ["test_blend_renamed"]
+    monkeypatch.setattr(KX, "COVERS", covers)
+    assert _entry_problems(HEADER) == [
+        "test_gpu_kernel_contract_ext.COVERS['yb_blend'] names a test that does not exist: test_blend_renamed"]
+    del covers["yb_blend"]
+    assert _entry_problems(HEADER) == ["entry point without a contract test: yb_blend"]
+
+
+# ------------------------------------------------------------------------------------------------------------
+# yb_vae_rms_act instance guard
+# ------------------------------------------------------------------------------------------------------------
+def _rms_problems(src, widths):
+    text = src.read_text()
+    problems = []
+    inst = {(int(n), int(g)) for n, g in re.findall(r"YB_RMS_LAUNCH\((\d+),\s*(\d+)\);", text)}
+    if not inst:
+        problems.append("no YB_RMS_LAUNCH instances found")
+    m1 = re.search(r"nch = C <= (\d+) \? 1 : \(C <= (\d+) \? 2 : 4\);", text)
+    m2 = re.search(r"g = nch > 1 \? 32 : \(Cp <= (\d+) \? 8 : \(Cp <= (\d+) \? 16 : 32\)\);", text)
+    if not (m1 and m2):
+        return problems + ["the width rule of yb_vae_rms_act was not found (update this guard with it)"]
+    c1, c2, p1, p2 = int(m1[1]), int(m1[2]), int(m2[1]), int(m2[2])
+    reached = set()
+    for C, Cp in widths:
+        nch = 1 if C <= c1 else (2 if C <= c2 else 4)
+        g = 32 if nch > 1 else (8 if Cp <= p1 else (16 if Cp <= p2 else 32))
+        if KX.rms_instance(C, Cp) != (nch, g):
+            problems.append(f"rms_instance({C}, {Cp}) = {KX.rms_instance(C, Cp)}, the kernel picks {(nch, g)}")
+        reached.add((nch, g))
+    for n, g in sorted(inst - reached):
+        problems.append(f"YB_RMS_LAUNCH({n}, {g}) is reached by no tested width")
+    return problems
+
+
+def test_every_rms_act_instance_has_a_tested_width():
+    assert _rms_problems(CSRC / "vae_elementwise.cu", KX.RMS_WIDTHS) == []
+
+
+def test_rms_act_guard_notices_a_dropped_width():
+    widths = tuple(w for w in KX.RMS_WIDTHS if w != (48, 64))
+    assert _rms_problems(CSRC / "vae_elementwise.cu", widths) == ["YB_RMS_LAUNCH(1, 8) is reached by no tested width"]
+
+
+# ------------------------------------------------------------------------------------------------------------
+# the new bounds reject their defects and accept the kernels' arithmetic
+# ------------------------------------------------------------------------------------------------------------
+def _masked_softmax_f32(S, L, hw, leak=0):
+    """fp32 frame-causal softmax as the kernel computes it (max, exp of the shifted logits, fp32 sum, 1/sum, bf16 out);
+    leak = 1 moves every frame boundary one key late (one next-frame key enters the row)."""
+    rows = torch.arange(S.shape[0])[:, None] // hw
+    cols = torch.arange(S.shape[1])[None, :]
+    keep = (cols < (torch.clamp((rows + 1) * hw + leak, max=L))) & (cols < L)
+    s = S.masked_fill(~keep, -math.inf)
+    e = torch.exp(s - s.amax(1, keepdim=True))
+    return (e * (1.0 / e.sum(1, keepdim=True))).bfloat16()
+
+
+def test_masked_softmax_bound_rejects_a_leaked_next_frame_key():
+    g = torch.Generator().manual_seed(11)
+    hw, L = 40, 115
+    S = torch.randn(L, 128, generator=g) * 8
+    p, f32, keep = KX.softmax_bound(S, L, hw)
+    bound = K.bf16_out_bound(p, f32)
+    assert K.assert_within(_masked_softmax_f32(S, L, hw), p, bound, "masked_softmax fp32") <= 1.0
+    with pytest.raises(AssertionError, match="out of bound"):
+        K.assert_within(_masked_softmax_f32(S, L, hw, leak=1), p, bound, "masked_softmax boundary one key late")
+
+
+def test_avgdown_bound_rejects_a_dropped_group_element():
+    g = torch.Generator().manual_seed(12)
+    T, H, W, in_c, out_c, ft, fs = 5, 4, 4, 64, 64, 2, 2
+    G = in_c * ft * fs * fs // out_c
+    x = torch.randn(T * H * W, in_c, generator=g).bfloat16()
+    m0 = torch.randn(3, 2, 2, out_c, generator=g).bfloat16()
+    mean, absmean = KX.avgdown_ref(x, (T, H, W), in_c, out_c, ft, fs)
+    ref = m0.double() + mean
+    bound = K.bf16_out_bound(ref, (G - 1) * K.U32 * absmean + K.U32 * ref.abs())
+    # the same grouping in fp32, as the kernel sums it: sequential over the G members, times the exact 1/G
+    xn = torch.nn.functional.pad(x.float().view(T, H, W, in_c).permute(3, 0, 1, 2)[None], (0, 0, 0, 0, 1, 0))
+    xn = xn.view(1, in_c, 3, ft, 2, fs, 2, fs).permute(0, 1, 3, 5, 7, 2, 4, 6).reshape(out_c, G, 3, 2, 2)
+    acc = torch.zeros(out_c, 3, 2, 2)
+    for j in range(G):
+        acc = acc + xn[:, j]
+    good = (m0.float() + (acc * (1.0 / G)).permute(1, 2, 3, 0)).bfloat16()
+    assert K.assert_within(good, ref, bound, "avgdown fp32") <= 1.0
+    bad = (m0.float() + ((acc - xn[:, G - 1]) * (1.0 / G)).permute(1, 2, 3, 0)).bfloat16()
+    with pytest.raises(AssertionError, match="out of bound"):
+        K.assert_within(bad, ref, bound, "avgdown one group element dropped")
+
+
+def test_zero_pad_conv_bound_rejects_replicate_padding_on_one_face():
+    g = torch.Generator().manual_seed(13)
+    T, H, W, Cp, co, taps = 2, 5, 6, 64, 32, (3, 3, 3)
+    x = (torch.randn(T, H, W, Cp, generator=g) + 1.0).bfloat16()
+    wt = (torch.randn(co, Cp, 3, 3, 3, generator=g) / math.sqrt(27 * Cp)).bfloat16()
+    acc, Fb, _ = KX._conv_ref(x, wt, taps)
+    bound = K.bf16_out_bound(acc, Fb + 4 * K.U32 * acc.abs())
+    xf = x.float().permute(3, 0, 1, 2)[None]
+    zero = torch.nn.functional.pad(xf, (1, 1, 1, 1, 2, 0))
+    good = torch.nn.functional.conv3d(zero, wt.float())[0].permute(1, 2, 3, 0).reshape(-1, co).bfloat16()
+    assert K.assert_within(good, acc, bound, "conv zero pad fp32") <= 1.0
+    rep = zero.clone()
+    rep[..., 0] = rep[..., 1]                                     # the left W face replicated instead of zero
+    bad = torch.nn.functional.conv3d(rep, wt.float())[0].permute(1, 2, 3, 0).reshape(-1, co).bfloat16()
+    with pytest.raises(AssertionError, match="out of bound"):
+        K.assert_within(bad, acc, bound, "conv replicate-padded left face")
+
+
+def test_n_split_check_rejects_a_straddling_tile_sent_to_the_wrong_chunk():
+    """W3 = 384, 256-column tiles: tile 1 covers columns 256..511, i.e. chunk 0 columns 256..383 and chunk 1 columns 0..127.
+    The defect stores that second half into chunk 2 instead (chunk 1 keeps its NaN poison there)."""
+    got, ref, bound = _gemm_case(M=64, N=4 * 384, Kd=128)
+    P, W3 = 4, 384
+    chunks = got.view(64, P, W3).permute(1, 0, 2).clone()              # [P, Lp, W3] as the kernel lays it out
+    assert K.assert_within(chunks.permute(1, 0, 2).reshape(64, P * W3), ref, bound, "n_split layout") <= 1.0
+    chunks[2, :, :128] = chunks[1, :, :128]
+    chunks[1, :, :128] = float("nan")
+    with pytest.raises(AssertionError, match="out of bound"):
+        K.assert_within(chunks.permute(1, 0, 2).reshape(64, P * W3), ref, bound, "n_split straddling tile misplaced")
+
+
+def test_sp_sums_bound_rejects_a_missing_head_block():
+    g = torch.Generator().manual_seed(14)
+    L, C = 16, 3072
+    q = torch.randn(L, C, generator=g).bfloat16()
+    xsq = q.double().pow(2).sum(1)
+    bound = KX.sumsq_bound(xsq, C)
+    sq = q.float().pow(2)
+    good = sq.view(L, C // 256, 256).sum(2).sum(1)                    # per-tile partials, then across tiles (fp32)
+    assert K.assert_within(good, xsq, bound, "sum q^2 fp32") <= 1.0
+    bad = good.clone()
+    bad[5] = sq[5, :C - 128].sum()
+    with pytest.raises(AssertionError, match=r"1 of 16 elements out of bound; worst at \(5,\)"):
+        K.assert_within(bad, xsq, bound, "sum q^2 without the last head block")

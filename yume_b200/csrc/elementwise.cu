@@ -828,7 +828,9 @@ extern "C" int yb_linear_f32_small(const void* in, const void* W, const void* bi
 extern "C" int yb_linear_f32(const void* in, long long ldi, const void* W, const void* bias, void* out, long long ldo,
                              int M, int N, int K, void* stream_) {
   if (!in || !W || !out || M <= 0 || N <= 0 || K <= 0) return YB_ERR_ARG;
-  if ((K % 4) || (ldi % 4)) return YB_ERR_SHAPE;
+  if ((K % 4) || (ldi % 4) || (N % 4)) return YB_ERR_SHAPE;
+  // the kernel reads `in` and `W` as float4
+  if ((reinterpret_cast<uintptr_t>(in) & 0xF) || (reinterpret_cast<uintptr_t>(W) & 0xF)) return YB_ERR_ALIGNMENT;
   dim3 grid((N + 63) / 64, (M + 63) / 64);
   linear_f32_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(in), ldi, static_cast<const float*>(W), static_cast<const float*>(bias),

@@ -197,8 +197,15 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, long long ldx, 
   }
 }
 
+// One cross-fade step of blend_v / blend_h / blend_t: `a * (1 - y / ext) + b * (y / ext)` on f32 tensors. Python computes both
+// weights in double and torch rounds them to f32; each product and the sum is rounded on its own (no fused multiply-add).
+__device__ __forceinline__ float xfade(float a, float b, int y, int ext) {
+  const double r = static_cast<double>(y) / static_cast<double>(ext);
+  return __fadd_rn(__fmul_rn(a, static_cast<float>(1.0 - r)), __fmul_rn(b, static_cast<float>(r)));
+}
+
 // cross-fade along one axis of contiguous f32 [C, T, H, W] tiles (blend_v / blend_h / blend_t):
-//   b[.., y, ..] = a[.., ea - ext + y, ..] * (1 - y/ext) + b[.., y, ..] * (y/ext)   for y < ext
+//   b[.., y, ..] = a[.., ea - ext + y, ..] * (1 - y/ext) + b[.., y, ..] * (y/ext)   for y < ext   (xfade: the reference's roundings)
 // a has extent `ea` on the blend axis, b has `eb`; all other extents equal. outer/inner: product of the dims before /
 // after the axis.
 __global__ void blend_kernel(const float* __restrict__ a, float* __restrict__ b, long long outer, int ea, int eb, int ext,
@@ -209,10 +216,9 @@ __global__ void blend_kernel(const float* __restrict__ a, float* __restrict__ b,
     const long long in = i % inner;
     const int y = static_cast<int>((i / inner) % ext);
     const long long o = i / (inner * ext);
-    const float wb = static_cast<float>(y) / static_cast<float>(ext);
     const float av = a[o * a_outer_stride + static_cast<long long>(ea - ext + y) * inner + in];
     float* bp = b + o * b_outer_stride + static_cast<long long>(y) * inner + in;
-    *bp = av * (1.f - wb) + *bp * wb;
+    *bp = xfade(av, *bp, y, ext);
   }
 }
 
@@ -247,12 +253,6 @@ __device__ __forceinline__ float tile_at(const TileAsm& a, int ti, int i, int j,
   const float* t = a.ptr[(ti * a.ni + i) * a.nj + j];
   const int skip = ti > 0 ? 1 : 0;   // later temporal tiles: the first decoded frame is dropped (dec[:, :, 1:], :519-520)
   return t[((static_cast<long long>(c) * (a.tlen[ti] + skip) + f + skip) * a.th[i] + y) * a.tw[j] + x];
-}
-// One cross-fade step of blend_v / blend_h / blend_t: `a * (1 - y / ext) + b * (y / ext)` on f32 tensors. Python computes both
-// weights in double and torch rounds them to f32; each product and the sum is rounded on its own (no fused multiply-add).
-__device__ __forceinline__ float xfade(float a, float b, int y, int ext) {
-  const double r = static_cast<double>(y) / static_cast<double>(ext);
-  return __fadd_rn(__fmul_rn(a, static_cast<float>(1.0 - r)), __fmul_rn(b, static_cast<float>(r)));
 }
 // fully blended value of spatial tile (i, j) of temporal tile ti at (y, x): blend_v with the upper neighbour first, then blend_h
 // with the left neighbour (the reference's order, :440-448); neighbours enter with THEIR blends applied, which for the rows /
