@@ -101,6 +101,11 @@ SIGNATURES = {
     "yb_umma_probe": (_i, [_vp, _vp, _vp, _i, _vp]),
 }
 
+# every symbol include/yume_b200_clip.h declares (the CLIP vision encoder's input kernel)
+CLIP_SIGNATURES = {
+    "yb_resize_bicubic_normalize": (_i, [_vp, _ll, _ll, _ll, _i, _i, _i, _vp, _i, _vp, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -121,7 +126,7 @@ def load():
     if lib.yb_abi_version() != ABI_VERSION:
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
-    for name, (res, args) in SIGNATURES.items():
+    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

@@ -14,6 +14,7 @@ from ._lib import (YB_ATT_ACCUMULATE, YB_ATT_P_SMEM, YB_EPI_BF16, YB_EPI_F32, YB
 
 __all__ = [
     "gemm", "ln_modulate", "rmsnorm_rope", "qk_norm_rope", "flop_count", "attention", "patchify", "unpatchify", "sinusoidal",
+    "resize_bicubic_normalize",
     "linear_f32_small", "linear_f32", "umma_probe", "launch_count", "reset_launch_count",
     "YB_EPI_BF16", "YB_EPI_GELU_BF16", "YB_EPI_F32", "YB_EPI_GATE_RES", "YB_EPI_GELU_ERF_BF16", "bcast_add",
     "YB_ATT_P_SMEM", "YB_ATT_ACCUMULATE",
@@ -240,6 +241,28 @@ def patchify(x: torch.Tensor, out: torch.Tensor, ph: int, pw: int) -> torch.Tens
     sc, sf, sh, sw = x.stride()
     check(_lib.load().yb_patchify(x.data_ptr(), sc, sf, sh, sw, out.data_ptr(), out.stride(0), Cin, F, H, W, ph, pw,
                                   _stream()), "yb_patchify")
+    _launches += 1
+    return out
+
+
+def resize_bicubic_normalize(x: torch.Tensor, out: torch.Tensor, mean: torch.Tensor, std: torch.Tensor) -> torch.Tensor:
+    """x f32 [C, H, W] (any strides) -> out f32 [C, S, S] contiguous: F.interpolate(bicubic, align_corners=False), then
+    * 0.5 + 0.5, - mean[c], / std[c] (mean, std f32 [C]); see include/yume_b200_clip.h."""
+    global _launches
+    if not x.is_cuda or x.dtype != torch.float32 or x.dim() != 3:
+        raise YumeB200Error("resize_bicubic_normalize input must be a CUDA float32 [C, H, W] tensor")
+    _need(out, torch.float32, "out")
+    Cn, H, W = x.shape
+    S = out.shape[-1]
+    if not out.is_contiguous() or tuple(out.shape) != (Cn, S, S):
+        raise YumeB200Error(f"resize_bicubic_normalize out must be a contiguous [{Cn}, S, S], got {tuple(out.shape)}")
+    for name, t in (("mean", mean), ("std", std)):
+        _need(t, torch.float32, name)
+        if t.numel() != Cn or not t.is_contiguous():
+            raise YumeB200Error(f"resize_bicubic_normalize {name} must be a contiguous f32 [{Cn}]")
+    sc, sh, sw = x.stride()
+    check(_lib.load().yb_resize_bicubic_normalize(x.data_ptr(), sc, sh, sw, Cn, H, W, out.data_ptr(), S, mean.data_ptr(),
+                                                  std.data_ptr(), _stream()), "yb_resize_bicubic_normalize")
     _launches += 1
     return out
 
