@@ -8,7 +8,12 @@
     exempt, with its reason), every test a table names exists, and a tested width reaches each YB_RMS_LAUNCH instance;
   * the bounds of tests/test_gpu_kernel_contract_ext.py reject their defects (a next-frame key leaking into a masked softmax
     row, an AvgDown group element dropped, replicate instead of zero padding on one conv face, a straddling n_split tile
-    sent to the wrong chunk, a token's sum of squares missing a head block) and accept the kernels' arithmetic.
+    sent to the wrong chunk, a token's sum of squares missing a head block) and accept the kernels' arithmetic;
+  * the production-shape table of tests/test_gpu_kernel_contract_prod.py stays multi-wave (planned at 132 SMs), with 5B and 14B
+    self-attention rows on the tail split; its sample sets hit every tile, conv box and (head, unit, query tile); and its sampled
+    checker rejects, at production M x N with a tiny K, a tile written with its neighbour's coordinates, a GATE_RES tile with the
+    wrong tok_idx row, KV tile 100 of 145 dropped in one unit the sampler covers by its per-tile rows only, and a unit whose second
+    query tile was never written.
 """
 import math
 import re
@@ -400,3 +405,179 @@ def test_sp_sums_bound_rejects_a_missing_head_block():
     bad[5] = sq[5, :C - 128].sum()
     with pytest.raises(AssertionError, match=r"1 of 16 elements out of bound; worst at \(5,\)"):
         K.assert_within(bad, xsq, bound, "sum q^2 without the last head block")
+
+
+# ------------------------------------------------------------------------------------------------------------
+# production-shape contract (tests/test_gpu_kernel_contract_prod.py): the table stays multi-wave, the sampler hits every
+# tile, and the sampled checker rejects cross-tile defects at production M x N
+# ------------------------------------------------------------------------------------------------------------
+import test_gpu_kernel_contract_prod as KP  # noqa: E402
+
+
+def _wave_problems(table):
+    problems = []
+    vae_cfgs = {r["cfg"] for r in table if r["entry"] == "conv"}
+    multi = set()
+    for r in table:
+        p = KP.row_plan(r)
+        if r["entry"] in ("attention", "attention_sp"):
+            if r.get("self_attn") and p["nkv"] < 100:
+                problems.append(f"{r['id']}: {p['nkv']} KV tiles < 100")
+            if not r.get("self_attn") and p["per_cta"] < 3:
+                problems.append(f"{r['id']}: {p['per_cta']:.2f} units per SM < 3")
+        elif p["per_cta"] >= 3:
+            multi.add(r["cfg"])
+            if r["id"] in KP.WAVE_EXEMPT:
+                problems.append(f"{r['id']}: exempt, but plans {p['per_cta']:.2f} tiles per CTA")
+        elif r["id"] not in KP.WAVE_EXEMPT:
+            problems.append(f"{r['id']}: {p['per_cta']:.2f} tiles per CTA < 3")
+    for cfg in sorted(vae_cfgs - multi):
+        problems.append(f"{cfg}: no conv / GEMM row with >= 3 tiles per CTA")
+    for tree in ("5b", "14b"):
+        if not any(r["entry"] == "attention" and r.get("self_attn") and r["cfg"].startswith(tree) and KP.row_plan(r)["tail"] > 0
+                   for r in table):
+            problems.append(f"no {tree} self-attention row takes the tail split")
+    if not any(r["entry"] == "gemm" and r.get("raster") and KP.row_plan(r)["n_tiles"] >= 100 * KP.row_plan(r)["m_tiles"]
+               for r in table):
+        problems.append("no raster row with >= 100 N tiles per M tile")
+    return problems
+
+
+def test_production_table_is_multi_wave():
+    assert _wave_problems(KP.PROD_TABLE) == []
+
+
+def test_multi_wave_guard_notices_a_shrunk_table():
+    t = KP.PROD_TABLE
+    no_split = [r for r in t if not (r["entry"] == "attention" and r["id"] == "5b.self_attention")]
+    assert _wave_problems(no_split) == ["no 5b self-attention row takes the tail split"]
+    short = [dict(r, L=2310, M=2310) if r["id"] == "5b.o" else r for r in t]
+    assert _wave_problems(short) == ["5b.o: 1.73 tiles per CTA < 3"]
+    short_kv = [dict(r, Lk=8000) if r["id"] == "14b_grid.self_attention" else r for r in t]
+    assert _wave_problems(short_kv) == ["14b_grid.self_attention: 63 KV tiles < 100"]
+    no_raster = [r for r in t if not r.get("raster")]
+    assert _wave_problems(no_raster) == ["no raster row with >= 100 N tiles per M tile"]
+    grown = [dict(r, T=9) if r["id"] == "hy_tile.conv9_2x64x64_512to512_k333" else r for r in t]
+    assert _wave_problems(grown) == ["hy_tile.conv9_2x64x64_512to512_k333: exempt, but plans 4.36 tiles per CTA"]
+
+
+def _sample_problems(table, gemm_sample=None):
+    gemm_sample = gemm_sample or KP.gemm_sample
+    problems = []
+    for r in table:
+        p = KP.row_plan(r)
+        if r["entry"] == "gemm":
+            rows, cols = gemm_sample(r["M"], r["N"], r["id"])
+            for bm in (128, 256):
+                miss = KP.gemm_tiles_missed(rows, cols, r["M"], r["N"], bm, p["block_n"])
+                if miss:
+                    problems.append(f"{r['id']}: {len(miss)} {bm}-row tiles without samples, first {miss[0]}")
+        elif r["entry"] == "gemm_sp_qkv":          # every rank's own 256-row SM-pair tiles and 256-wide N tiles
+            rows, cols = KP.gemm_sp_qkv_sample(r)
+            for rank in range(r["P"]):
+                mine = rows[(rows // r["Lp"]) == rank] - rank * r["Lp"]
+                miss = KP.gemm_tiles_missed(mine, cols, r["Lp"], 3 * r["C"], p["block_m"], p["block_n"])
+                if miss:
+                    problems.append(f"{r['id']}: rank {rank}: {len(miss)} tiles without samples, first {miss[0]}")
+        elif r["entry"] == "conv":
+            miss = KP.conv_boxes_missed(KP.conv_sample(p["dims"], p["box"], r["id"]), p["dims"], p["box"])
+            if miss:
+                problems.append(f"{r['id']}: {len(miss)} boxes without samples")
+        elif r["entry"] in ("attention", "attention_sp"):
+            miss = KP.attention_units_missed(KP.attention_sample(p["Lq"], p["heads"], r["id"]), p["Lq"], p["heads"])
+            if miss:
+                problems.append(f"{r['id']}: {len(miss)} (head, unit, query tile) without samples, first {miss[0]}")
+    return problems
+
+
+def test_sampler_hits_every_tile_box_and_unit():
+    assert _sample_problems(KP.PROD_TABLE) == []
+
+
+def test_sampler_guard_notices_a_band_without_samples():
+    def broken(M, N, key):                                   # the rows of band 5 never sampled
+        rows, cols = KP.gemm_sample(M, N, key)
+        return rows[(rows // 128) != 5], cols[(cols // 256) != 3]
+    rows = [r for r in KP.PROD_TABLE if r["id"] == "5b.qkv"]
+    probs = _sample_problems(rows, broken)
+    assert probs and "5b.qkv: 1 128-row tiles without samples, first (5, 3)" in probs[0]
+
+
+def _prod_gemm_case(gated=False):
+    """Production M x N (the 5B o-projection) with K = 16, computed the way the kernel does (fp32 accumulation)."""
+    g = torch.Generator().manual_seed(21)
+    M, N, Kd = 18480, 3072, 16
+    A = torch.randn(M, Kd, generator=g).bfloat16()
+    B = (torch.randn(N, Kd, generator=g) / 4).bfloat16()
+    bias = torch.randn(N, generator=g)
+    acc = A.float() @ B.float().t() + bias
+    if not gated:
+        return A, B, bias, acc, None
+    gate6 = torch.randn(2, 6, N, generator=g)
+    tok = (torch.arange(M) >= M // 3).long()
+    return A, B, bias, acc, (gate6, tok)
+
+
+@pytest.mark.parametrize("tile", [(0, 4), (77, 5), (144, 11)])     # first band, interior, last (partial: 48 rows) band
+def test_prod_gemm_check_rejects_a_tile_written_with_its_neighbours_coordinates(tile):
+    A, B, bias, acc, _ = _prod_gemm_case()
+    got = acc.bfloat16()
+    rows, cols = KP.gemm_sample(A.shape[0], B.shape[0], "defect")
+    KP._check_gemm_sampled(got, A, B, rows, cols, KP.EPI["BF16"], "kernel arithmetic", None, bias=bias)
+    i, j = tile
+    jn = j + 1 if j + 1 < 12 else j - 1
+    rs = slice(i * 128, min((i + 1) * 128, A.shape[0]))
+    got[rs, j * 256:(j + 1) * 256] = got[rs, jn * 256:(jn + 1) * 256]
+    with pytest.raises(AssertionError, match="out of bound"):
+        KP._check_gemm_sampled(got, A, B, rows, cols, KP.EPI["BF16"], f"tile {tile} from its neighbour", None, bias=bias)
+
+
+def test_prod_gemm_check_rejects_a_gate_res_tile_with_the_wrong_tok_idx_row():
+    A, B, bias, acc, (gate6, tok) = _prod_gemm_case(gated=True)
+    x0 = torch.randn(acc.shape, generator=torch.Generator().manual_seed(3))
+    gate_rows = lambda ri: gate6[tok[ri if ri is not None else slice(None)], 2].double()      # noqa: E731
+    good = x0 + acc * gate6[tok, 2]
+    rows, cols = KP.gemm_sample(A.shape[0], B.shape[0], "defect")
+    KP._check_gemm_sampled(good, A, B, rows, cols, KP.EPI["GATE_RES"], "GATE_RES kernel arithmetic", None, bias=bias, x0=x0,
+                           gate_rows=gate_rows)
+    bad = good.clone()
+    rs, cs = slice(10 * 128, 11 * 128), slice(3 * 256, 4 * 256)          # a tile of history tokens used the new-token gate
+    bad[rs, cs] = x0[rs, cs] + acc[rs, cs] * gate6[1, 2, cs]
+    with pytest.raises(AssertionError, match="out of bound"):
+        KP._check_gemm_sampled(bad, A, B, rows, cols, KP.EPI["GATE_RES"], "GATE_RES wrong tok_idx row", None, bias=bias, x0=x0,
+                               gate_rows=gate_rows)
+
+
+def _prod_attention_case(seed, drop_unit=None, Lq=1024, Lk=18480):
+    """One head, Lq = 1024 (4 units), Lk = 18480 (145 KV tiles), data drawn like the GPU test's (q * 2, unit-variance k and v)
+    and computed as the kernel does (fp32 logits and softmax, P in bf16, fp32 normaliser, bf16 out). drop_unit: KV tile 100
+    is missing from every row of that unit."""
+    g = torch.Generator().manual_seed(seed)
+    q = (torch.randn(Lq, 128, generator=g) * 2).bfloat16()
+    k, v = torch.randn(Lk, 128, generator=g).bfloat16(), torch.randn(Lk, 128, generator=g).bfloat16()
+    scale = 1 / math.sqrt(128.0)
+    s = (q.float() @ k.float().t()) * scale
+    if drop_unit is not None:
+        s[drop_unit * 256:(drop_unit + 1) * 256, 100 * 128:101 * 128] = -math.inf
+    p = torch.exp(s - s.amax(-1, keepdim=True))
+    got = ((p.bfloat16().float() @ v.float()) / p.sum(-1, keepdim=True)).bfloat16()
+    return got, q, k, v, scale, dict(nkv=-(-Lk // 128), ns=1)
+
+
+@pytest.mark.parametrize("seed", [0, 1, 2, 3])
+def test_prod_attention_check_rejects_kv_tile_100_dropped_in_one_unit(seed):
+    """The dropped tile is in a unit the sampler covers with its per-tile rows only (not the one whole unit per head)."""
+    key = ("defect", seed)
+    whole = int(torch.bincount(KP.attention_sample(1024, 1, key)[0] // 256).argmax())
+    got, q, k, v, scale, plan = _prod_attention_case(seed)
+    KP._check_attention_sampled(got, q, k, v, 1, scale, plan, key, "kernel arithmetic", None)
+    got, q, k, v, scale, plan = _prod_attention_case(seed, drop_unit=(whole + 1) % 4)
+    with pytest.raises(AssertionError, match=r"head0: \d+ of \d+ elements out of bound"):
+        KP._check_attention_sampled(got, q, k, v, 1, scale, plan, key, "KV tile 100 dropped in one unit", None)
+
+
+def test_prod_attention_check_rejects_a_tail_unit_with_an_unwritten_second_query_tile():
+    got, q, k, v, scale, plan = _prod_attention_case(0)
+    got[768 + 128:1024] = float("nan")                         # the last unit's second 128-row query tile
+    with pytest.raises(AssertionError, match=r"\|err\|/bound = inf"):
+        KP._check_attention_sampled(got, q, k, v, 1, scale, plan, "defect", "second query tile never written", None)
