@@ -106,6 +106,13 @@ CLIP_SIGNATURES = {
     "yb_resize_bicubic_normalize": (_i, [_vp, _ll, _ll, _ll, _i, _i, _i, _vp, _i, _vp, _vp, _vp]),
 }
 
+# every symbol include/yume_b200_t5.h declares (the umT5 text encoder's attention, RMS norm and gated GELU)
+T5_SIGNATURES = {
+    "yb_t5_attention": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _i, _vp, _vp, _vp]),
+    "yb_t5_rmsnorm": (_i, [_vp, _ll, _vp, _ll, _i, _vp, _i, _i, _f, _vp]),
+    "yb_t5_geglu": (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
+}
+
 _lib = None
 
 
@@ -126,7 +133,7 @@ def load():
     if lib.yb_abi_version() != ABI_VERSION:
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
-    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES}.items():
+    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

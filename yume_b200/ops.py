@@ -14,7 +14,7 @@ from ._lib import (YB_ATT_ACCUMULATE, YB_ATT_P_SMEM, YB_EPI_BF16, YB_EPI_F32, YB
 
 __all__ = [
     "gemm", "ln_modulate", "rmsnorm_rope", "qk_norm_rope", "flop_count", "attention", "patchify", "unpatchify", "sinusoidal",
-    "resize_bicubic_normalize",
+    "resize_bicubic_normalize", "t5_attention", "t5_rmsnorm", "t5_geglu",
     "linear_f32_small", "linear_f32", "umma_probe", "launch_count", "reset_launch_count",
     "YB_EPI_BF16", "YB_EPI_GELU_BF16", "YB_EPI_F32", "YB_EPI_GATE_RES", "YB_EPI_GELU_ERF_BF16", "bcast_add",
     "YB_ATT_P_SMEM", "YB_ATT_ACCUMULATE",
@@ -263,6 +263,63 @@ def resize_bicubic_normalize(x: torch.Tensor, out: torch.Tensor, mean: torch.Ten
     sc, sh, sw = x.stride()
     check(_lib.load().yb_resize_bicubic_normalize(x.data_ptr(), sc, sh, sw, Cn, H, W, out.data_ptr(), S, mean.data_ptr(),
                                                   std.data_ptr(), _stream()), "yb_resize_bicubic_normalize")
+    _launches += 1
+    return out
+
+
+def t5_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor, out: torch.Tensor, B: int, heads: int,
+                 bias: torch.Tensor, key_mask: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """T5 self-attention (no scale, relative-position bias, key padding mask), head_dim 64. q, k, v, out bf16
+    [B*L, heads*64] (row strides arbitrary); bias f32 [heads, 2L-1] contiguous; key_mask uint8 [B, L] contiguous (nonzero =
+    attend) or None; see include/yume_b200_t5.h."""
+    global _launches, _flops
+    for n, t in (("q", q), ("k", k), ("v", v), ("out", out)):
+        _need(t, torch.bfloat16, n)
+    BL = q.shape[0]
+    if BL % B or any(t.shape != (BL, heads * 64) for t in (q, k, v, out)):
+        raise YumeB200Error(f"t5_attention: q, k, v, out must be [B*L, {heads * 64}] with B = {B}")
+    L = BL // B
+    _need(bias, torch.float32, "bias")
+    if tuple(bias.shape) != (heads, 2 * L - 1) or not bias.is_contiguous():
+        raise YumeB200Error(f"t5_attention: bias must be a contiguous f32 [{heads}, {2 * L - 1}]")
+    if key_mask is not None:
+        if not key_mask.is_cuda or key_mask.dtype != torch.uint8 or tuple(key_mask.shape) != (B, L) or \
+                not key_mask.is_contiguous():
+            raise YumeB200Error(f"t5_attention: key_mask must be a contiguous CUDA uint8 [{B}, {L}]")
+    check(_lib.load().yb_t5_attention(q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0), v.data_ptr(), v.stride(0),
+                                      out.data_ptr(), out.stride(0), B, L, heads, bias.data_ptr(), _ptr(key_mask),
+                                      _stream()), "yb_t5_attention")
+    _launches += 1
+    _flops += 4.0 * B * L * L * heads * 64
+    return out
+
+
+def t5_rmsnorm(x: torch.Tensor, out: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
+    """out = x * rsqrt(mean(x^2) + eps) * weight (T5LayerNorm); x f32 [L, C]; out bf16 or f32 [L, C]; weight f32 [C]."""
+    global _launches
+    _need(x, torch.float32, "x")
+    L, Cdim = x.shape
+    out_f32 = 1 if out.dtype == torch.float32 else 0
+    _need(out, torch.float32 if out_f32 else torch.bfloat16, "out")
+    _need(weight, torch.float32, "weight")
+    if tuple(out.shape) != (L, Cdim) or weight.numel() != Cdim or not weight.is_contiguous():
+        raise YumeB200Error(f"t5_rmsnorm: out must be [{L}, {Cdim}] and weight a contiguous f32 [{Cdim}]")
+    check(_lib.load().yb_t5_rmsnorm(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), out_f32, weight.data_ptr(),
+                                    L, Cdim, eps, _stream()), "yb_t5_rmsnorm")
+    _launches += 1
+    return out
+
+
+def t5_geglu(ug: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """out bf16 [L, F] = u * gelu_tanh(g) with ug bf16 [L, 2F] = [u | g] (fc1 columns, then gate columns)."""
+    global _launches
+    _need(ug, torch.bfloat16, "ug")
+    _need(out, torch.bfloat16, "out")
+    L, F2 = ug.shape
+    if F2 % 2 or tuple(out.shape) != (L, F2 // 2):
+        raise YumeB200Error(f"t5_geglu: ug must be [L, 2F] and out [L, F], got {tuple(ug.shape)} and {tuple(out.shape)}")
+    check(_lib.load().yb_t5_geglu(ug.data_ptr(), ug.stride(0), out.data_ptr(), out.stride(0), L, F2 // 2, _stream()),
+          "yb_t5_geglu")
     _launches += 1
     return out
 
