@@ -113,6 +113,16 @@ T5_SIGNATURES = {
     "yb_t5_geglu": (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
 }
 
+# every symbol include/yume_b200_stream.h declares (the chunk-streaming forms of the Wan VAE kernels)
+STREAM_SIGNATURES = {
+    "yb_conv3d_causal_hist": (_i, [C.POINTER(Conv3dArgs), _i, _vp]),
+    "yb_vae_dupup_add_cont": (_i, [_vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "yb_vae_unpatchify2_clamp_win": (_i, [_vp, _ll, _vp, _ll, _i, _i, _i, _vp]),
+    "yb_nhwc_to_nchw_f32_clamp_win": (_i, [_vp, _ll, _vp, _ll, _ll, _i, _f, _f, _vp]),
+    "yb_vae_patchify2_bf16_win": (_i, [_vp, _ll, _vp, _ll, _i, _i, _i, _vp]),
+    "yb_nchw_to_nhwc_bf16_win": (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
+}
+
 _lib = None
 
 
@@ -133,7 +143,7 @@ def load():
     if lib.yb_abi_version() != ABI_VERSION:
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
-    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES}.items():
+    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

@@ -20,6 +20,7 @@
 // The SM-pair form (CLUSTER = 2) is a cluster of two CTAs that owns a 256 x block_n tile: each CTA loads its own 128 rows of A
 // and HALF of the B tile, and multicasts that half into both CTAs, so the B operand crosses L2 once per pair of SMs.
 #include "yb_host.h"
+#include "../../include/yume_b200_stream.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -884,11 +885,14 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
 
 
 // Causal 3x3x3 conv (replicate padding) as an implicit GEMM on the same kernel. See include/yume_b200.h.
-extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
+// t_hist > 0 is the history form (include/yume_b200_stream.h): the input holds t_hist carried frames in front of the T new ones,
+// and those frames take the place of the causal zero padding in time (the tensor map spans all t_hist + T frames).
+static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
   using namespace yb;
   if (!a || !a->xpad || !a->w || !a->out) return YB_ERR_ARG;
   if (a->struct_bytes != sizeof(yb_conv3d_args)) return YB_ERR_ARG;
   if (a->T <= 0 || a->H <= 0 || a->W <= 0 || a->Cp <= 0 || a->Cout <= 0) return YB_ERR_ARG;
+  if (t_hist < 0) return YB_ERR_ARG;
   if (a->Cp % 64 != 0 || a->Cout % 32 != 0) return YB_ERR_SHAPE;
   if ((a->ldo % 8) || (reinterpret_cast<uintptr_t>(a->out) & 0xF)) return YB_ERR_ALIGNMENT;
   if (a->epilogue != YB_EPI_BF16 && a->epilogue != YB_EPI_F32 && a->epilogue != YB_EPI_RES_BF16) return YB_ERR_ARG;
@@ -906,8 +910,11 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
   if (st_t > 2 || st_hw > 2) return YB_ERR_ARG;
   const bool strided = st_t > 1 || st_hw > 1;
   if (strided && !a->oob_zero_pad) return YB_ERR_ARG;
+  // history: exactly the kt-1 frames of the causal pad (unit stride), or the one frame the stride-2 time_conv carries
+  if (t_hist > 0 && (!a->oob_zero_pad || t_hist != (st_t > 1 ? 1 : kt - 1))) return YB_ERR_ARG;
+  const int inT = a->T + t_hist;   // frames the tensor map spans
   int oT = a->T, oH = a->H, oW = a->W;
-  if (st_t > 1) oT = (a->T - kt) / st_t + 1;
+  if (st_t > 1) oT = (inT - kt) / st_t + 1;
   if (st_hw > 1) { oH = (a->H + 1 - kh) / st_hw + 1; oW = (a->W + 1 - kw) / st_hw + 1; }
   if (oT <= 0 || oH <= 0 || oW <= 0) return YB_ERR_SHAPE;
   // SM-pair kernel: 1 = forced; 0 (automatic) and 2 run the 1-CTA kernel, the faster of the two on the H100 (see yb_gemm_plan)
@@ -922,7 +929,7 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
   p.cT = oT; p.cH = oH; p.cW = oW;
   p.kh = kh; p.kw = kw;
   p.st_t = st_t; p.st_h = st_hw; p.st_w = st_hw;
-  p.off_t = (a->oob_zero_pad && st_t == 1) ? kt - 1 : 0;
+  p.off_t = (a->oob_zero_pad && st_t == 1) ? kt - 1 - t_hist : 0;
   p.off_h = (a->oob_zero_pad && st_hw == 1) ? kh / 2 : 0;
   p.off_w = (a->oob_zero_pad && st_hw == 1) ? kw / 2 : 0;
   p.out_t_mul = a->out_t_mul > 0 ? a->out_t_mul : 1;
@@ -940,7 +947,7 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
   p.res_ld = a->res_ld;
   CUtensorMap tmA, tmB;
   const int padT = a->oob_zero_pad ? 0 : kt - 1, padH = a->oob_zero_pad ? 0 : kh - 1, padW = a->oob_zero_pad ? 0 : kw - 1;
-  int rc = make_tmap_bf16_4d(&tmA, a->xpad, a->T + padT, a->H + padH, a->W + padW, a->Cp, p.TT, p.TH,
+  int rc = make_tmap_bf16_4d(&tmA, a->xpad, inT + padT, a->H + padH, a->W + padW, a->Cp, p.TT, p.TH,
                              fuse_w ? CONVW_ROWS : p.TW, 64, st_t, st_hw, st_hw);
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmB, a->w, a->Cout, static_cast<uint64_t>(taps) * a->Cp, static_cast<uint64_t>(taps) * a->Cp,
@@ -973,4 +980,11 @@ extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream_) {
     YB_CONV_DISPATCH(0)
   }
 #undef YB_CONV_DISPATCH
+}
+
+extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream) { return conv3d_launch(a, 0, stream); }
+
+extern "C" int yb_conv3d_causal_hist(const yb_conv3d_args* a, int t_hist, void* stream) {
+  if (t_hist <= 0) return YB_ERR_ARG;
+  return conv3d_launch(a, t_hist, stream);
 }

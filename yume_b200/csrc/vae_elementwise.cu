@@ -6,6 +6,7 @@
 //   masked_softmax    frame-causal softmax of the mid-block attention scores (:37-45, diffusers Attention)
 //   layout converters and the tile cross-fade (autoencoder_kl_causal_3d.py:343-359)
 #include "yb_host.h"
+#include "../../include/yume_b200_stream.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -173,27 +174,27 @@ masked_softmax_kernel(const float* __restrict__ S, long long ldS, __nv_bfloat16*
     pr[j] = __float2bfloat16_rn(j < nvalid ? __expf(s[j] - mx) * inv : 0.f);
 }
 
-// z f32 [Cn, N] (NCDHW, N = T*H*W) -> bf16 [N, ldo] channels-last, columns >= Cn zero
+// z f32 [Cn, N] (NCDHW, N = T*H*W; channel planes `plane` elements apart) -> bf16 [N, ldo] channels-last, columns >= Cn zero
 __global__ void nchw_to_nhwc_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, long long N, int Cn,
-                                    int ldo) {
+                                    int ldo, long long plane) {
   const long long total = N * ldo;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const int c = static_cast<int>(i % ldo);
     const long long v = i / ldo;
-    out[i] = __float2bfloat16_rn(c < Cn ? x[static_cast<long long>(c) * N + v] : 0.f);
+    out[i] = __float2bfloat16_rn(c < Cn ? x[static_cast<long long>(c) * plane + v] : 0.f);
   }
 }
 
-// x f32 [N, ldx] channels-last -> out f32 [Cn, N]
+// x f32 [N, ldx] channels-last -> out f32 [Cn, N], channel planes `plane` elements apart (N for a dense result)
 __global__ void nhwc_to_nchw_kernel(const float* __restrict__ x, long long ldx, float* __restrict__ out, long long N,
-                                    int Cn, float lo, float hi) {
+                                    int Cn, float lo, float hi, long long plane) {
   const long long total = N * Cn;
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
     const long long v = i % N;
     const int c = static_cast<int>(i / N);
-    out[i] = fminf(fmaxf(x[v * ldx + c], lo), hi);
+    out[c * plane + v] = fminf(fmaxf(x[v * ldx + c], lo), hi);
   }
 }
 
@@ -403,14 +404,14 @@ rms_act_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16
 }
 
 // main[f', h', w', oc] += x[t, h, w, ci]: the DupUp3D shortcut (:376-418) of Up_ResidualBlock (:499-503) on the whole
-// sequence, first ft-1 duplicated frames dropped. d = f' + ft - 1, t = d / ft, a = d % ft, e = ((oc*ft + a)*fs + b)*fs + c,
-// ci = e / rep with rep = out_c*ft*fs*fs / in_c.
+// sequence, first `drop` duplicated frames dropped (ft-1 on the first chunk of a sequence, 0 on the chunks after it).
+// d = f' + drop, t = d / ft, a = d % ft, e = ((oc*ft + a)*fs + b)*fs + c, ci = e / rep with rep = out_c*ft*fs*fs / in_c.
 __global__ void __launch_bounds__(256)
 dupup_add_kernel(__nv_bfloat16* __restrict__ main_, const __nv_bfloat16* __restrict__ x, int Ts, int Hs, int Ws, int in_c,
-                 int out_c, int ft, int fs) {
+                 int out_c, int ft, int fs, int drop) {
   // one thread = 8 consecutive output channels of one output voxel: a 16-byte read-modify-write of main, eight gathers
   // from the (8x..16x smaller, cache-resident) source voxel
-  const int To = ft * Ts - (ft - 1), Ho = Hs * fs, Wo = Ws * fs;
+  const int To = ft * Ts - drop, Ho = Hs * fs, Wo = Ws * fs;
   const int rep = out_c * ft * fs * fs / in_c;
   const int rsh = (rep & (rep - 1)) == 0 ? 31 - __clz(rep) : -1;   // rep is 2, 4 or 8 in both Wan VAEs: shift, no division
   const int chunks = out_c >> 3;
@@ -424,7 +425,7 @@ dupup_add_kernel(__nv_bfloat16* __restrict__ main_, const __nv_bfloat16* __restr
     const int r = v / Wo;
     const int ho = r % Ho;
     const int fo = r / Ho;
-    const int d = fo + ft - 1;
+    const int d = fo + drop;
     const int t = d / ft, a = d % ft;
     const int e0 = ((oc * ft + a) * fs + (ho % fs)) * fs + (wo % fs);
     const __nv_bfloat16* xs = x + ((static_cast<long long>(t) * Hs + ho / fs) * Ws + wo / fs) * in_c;
@@ -487,7 +488,7 @@ avgdown_add_kernel(__nv_bfloat16* __restrict__ main_, const __nv_bfloat16* __res
 // video f32 [3, T, H, W] -> out bf16 [T*(H/2)*(W/2), ldo], channel (c r q) = c*4 + r*2 + q <- video[c, f, 2h + q, 2w + r]
 // (patchify 'b c f (h q) (w r) -> b (c r q) f h w', vae2_2.py:284-300); columns 12..ldo-1 are zeroed (TMA reads 64-channel chunks)
 __global__ void patchify2_bf16_kernel(const float* __restrict__ video, __nv_bfloat16* __restrict__ out, long long ldo, int T,
-                                      int H, int W) {
+                                      int H, int W, long long plane) {
   const int Hh = H / 2, Wh = W / 2;
   const long long total = static_cast<long long>(T) * Hh * Wh;
   for (long long v = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; v < total;
@@ -499,7 +500,7 @@ __global__ void patchify2_bf16_kernel(const float* __restrict__ video, __nv_bflo
     __nv_bfloat16* o = out + v * ldo;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
-      const float* src = video + ((static_cast<long long>(c) * T + f) * H + 2 * h) * W + 2 * w;
+      const float* src = video + c * plane + (static_cast<long long>(f) * H + 2 * h) * W + 2 * w;
       const float2 top = *reinterpret_cast<const float2*>(src);          // q = 0: r = 0, 1
       const float2 bot = *reinterpret_cast<const float2*>(src + W);      // q = 1
       o[c * 4 + 0] = __float2bfloat16_rn(top.x);   // r = 0, q = 0
@@ -514,7 +515,7 @@ __global__ void patchify2_bf16_kernel(const float* __restrict__ video, __nv_bflo
 // y f32 [T*H*W, ldy] (12 valid channels) -> out f32 [3, T, 2H, 2W], clamp to [-1, 1]:
 // unpatchify 'b (c r q) f h w -> b c f (h q) (w r)' (:305-319) + Wan2_2_VAE.decode's clamp_ (:1066-1067)
 __global__ void unpatchify2_clamp_kernel(const float* __restrict__ y, long long ldy, float* __restrict__ out, int T, int H,
-                                         int W) {
+                                         int W, long long plane) {
   const long long total = 3LL * T * (2 * H) * (2 * W);
   for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
        i += static_cast<long long>(gridDim.x) * blockDim.x) {
@@ -526,7 +527,7 @@ __global__ void unpatchify2_clamp_kernel(const float* __restrict__ y, long long 
     const int c = static_cast<int>(v / T);
     const int q = ho & 1, r = wo & 1;
     const float val = y[((static_cast<long long>(f) * H + (ho >> 1)) * W + (wo >> 1)) * ldy + (c * 2 + r) * 2 + q];
-    out[i] = fminf(fmaxf(val, -1.f), 1.f);
+    out[c * plane + (i - static_cast<long long>(c) * T * (2 * H) * (2 * W))] = fminf(fmaxf(val, -1.f), 1.f);
   }
 }
 
@@ -586,17 +587,21 @@ extern "C" int yb_masked_softmax(const void* S, long long ldS, void* P, long lon
   return check_launch("masked_softmax");
 }
 
-extern "C" int yb_nchw_to_nhwc_bf16(const void* x, void* out, long long N, int Cn, int ldo, void* stream_) {
-  if (!x || !out || N <= 0 || Cn <= 0 || ldo < Cn) return YB_ERR_ARG;
+extern "C" int yb_nchw_to_nhwc_bf16_win(const void* x, long long plane, void* out, long long N, int Cn, int ldo, void* stream_) {
+  if (!x || !out || N <= 0 || Cn <= 0 || ldo < Cn || plane < N) return YB_ERR_ARG;
   nchw_to_nhwc_kernel<<<grid_for(N * ldo), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      static_cast<const float*>(x), static_cast<__nv_bfloat16*>(out), N, Cn, ldo);
+      static_cast<const float*>(x), static_cast<__nv_bfloat16*>(out), N, Cn, ldo, plane);
   return check_launch("nchw_to_nhwc");
+}
+
+extern "C" int yb_nchw_to_nhwc_bf16(const void* x, void* out, long long N, int Cn, int ldo, void* stream_) {
+  return yb_nchw_to_nhwc_bf16_win(x, N, out, N, Cn, ldo, stream_);
 }
 
 extern "C" int yb_nhwc_to_nchw_f32(const void* x, long long ldx, void* out, long long N, int Cn, void* stream_) {
   if (!x || !out || N <= 0 || Cn <= 0 || ldx < Cn) return YB_ERR_ARG;
   nhwc_to_nchw_kernel<<<grid_for(N * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, -INFINITY, INFINITY);
+      static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, -INFINITY, INFINITY, N);
   return check_launch("nhwc_to_nchw");
 }
 
@@ -604,7 +609,7 @@ extern "C" int yb_nhwc_to_nchw_f32_clamp(const void* x, long long ldx, void* out
                                          void* stream_) {
   if (!x || !out || N <= 0 || Cn <= 0 || ldx < Cn || !(lo <= hi)) return YB_ERR_ARG;
   nhwc_to_nchw_kernel<<<grid_for(N * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, lo, hi);
+      static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, lo, hi, N);
   return check_launch("nhwc_to_nchw_clamp");
 }
 
@@ -666,16 +671,27 @@ extern "C" int yb_vae_rms_act(const void* x, long long ldx, void* out, const voi
   return check_launch("vae_rms_act");
 }
 
-extern "C" int yb_vae_dupup_add(void* main_, const void* x, int Ts, int Hs, int Ws, int in_c, int out_c, int ft, int fs,
-                                void* stream_) {
+static int dupup_launch(void* main_, const void* x, int Ts, int Hs, int Ws, int in_c, int out_c, int ft, int fs, bool first,
+                        void* stream_) {
   if (!main_ || !x || Ts <= 0 || Hs <= 0 || Ws <= 0 || in_c <= 0 || out_c <= 0 || ft < 1 || fs < 1) return YB_ERR_ARG;
   if ((out_c * ft * fs * fs) % in_c != 0 || out_c % 8 != 0) return YB_ERR_SHAPE;
   if (reinterpret_cast<uintptr_t>(main_) & 0xF) return YB_ERR_ALIGNMENT;
-  if (static_cast<long long>(ft * Ts - (ft - 1)) * Hs * fs * Ws * fs > 0x7fffffffLL) return YB_ERR_SHAPE;
-  const long long total = static_cast<long long>(ft * Ts - (ft - 1)) * Hs * fs * Ws * fs * (out_c / 8);
+  const int drop = first ? ft - 1 : 0;
+  if (static_cast<long long>(ft * Ts - drop) * Hs * fs * Ws * fs > 0x7fffffffLL) return YB_ERR_SHAPE;
+  const long long total = static_cast<long long>(ft * Ts - drop) * Hs * fs * Ws * fs * (out_c / 8);
   dupup_add_kernel<<<grid_for(total), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      static_cast<__nv_bfloat16*>(main_), static_cast<const __nv_bfloat16*>(x), Ts, Hs, Ws, in_c, out_c, ft, fs);
+      static_cast<__nv_bfloat16*>(main_), static_cast<const __nv_bfloat16*>(x), Ts, Hs, Ws, in_c, out_c, ft, fs, drop);
   return check_launch("vae_dupup_add");
+}
+
+extern "C" int yb_vae_dupup_add(void* main_, const void* x, int Ts, int Hs, int Ws, int in_c, int out_c, int ft, int fs,
+                                void* stream_) {
+  return dupup_launch(main_, x, Ts, Hs, Ws, in_c, out_c, ft, fs, true, stream_);
+}
+
+extern "C" int yb_vae_dupup_add_cont(void* main_, const void* x, int Ts, int Hs, int Ws, int in_c, int out_c, int ft, int fs,
+                                     void* stream_) {
+  return dupup_launch(main_, x, Ts, Hs, Ws, in_c, out_c, ft, fs, false, stream_);
 }
 
 extern "C" int yb_vae_avgdown_add(void* main_, const void* x, int T, int H, int W, int in_c, int out_c, int ft, int fs,
@@ -691,19 +707,38 @@ extern "C" int yb_vae_avgdown_add(void* main_, const void* x, int T, int H, int 
   return check_launch("vae_avgdown_add");
 }
 
-extern "C" int yb_vae_patchify2_bf16(const void* video, void* out, long long ldo, int T, int H, int W, void* stream_) {
+extern "C" int yb_vae_patchify2_bf16_win(const void* video, long long plane, void* out, long long ldo, int T, int H, int W,
+                                         void* stream_) {
   if (!video || !out || T <= 0 || H <= 0 || W <= 0 || ldo < 12) return YB_ERR_ARG;
   if ((H % 2) || (W % 2)) return YB_ERR_SHAPE;
-  if (reinterpret_cast<uintptr_t>(video) & 0x7) return YB_ERR_ALIGNMENT;
+  if (plane < static_cast<long long>(T) * H * W) return YB_ERR_ARG;
+  if ((reinterpret_cast<uintptr_t>(video) & 0x7) || (plane % 2)) return YB_ERR_ALIGNMENT;
   patchify2_bf16_kernel<<<grid_for(static_cast<long long>(T) * (H / 2) * (W / 2)), 256, 0,
                           reinterpret_cast<cudaStream_t>(stream_)>>>(static_cast<const float*>(video),
-                                                                     static_cast<__nv_bfloat16*>(out), ldo, T, H, W);
+                                                                     static_cast<__nv_bfloat16*>(out), ldo, T, H, W, plane);
   return check_launch("vae_patchify2_bf16");
 }
 
-extern "C" int yb_vae_unpatchify2_clamp(const void* y, long long ldy, void* out, int T, int H, int W, void* stream_) {
-  if (!y || !out || T <= 0 || H <= 0 || W <= 0 || ldy < 12) return YB_ERR_ARG;
+extern "C" int yb_vae_patchify2_bf16(const void* video, void* out, long long ldo, int T, int H, int W, void* stream_) {
+  return yb_vae_patchify2_bf16_win(video, static_cast<long long>(T) * H * W, out, ldo, T, H, W, stream_);
+}
+
+extern "C" int yb_vae_unpatchify2_clamp_win(const void* y, long long ldy, void* out, long long plane, int T, int H, int W,
+                                            void* stream_) {
+  if (!y || !out || T <= 0 || H <= 0 || W <= 0 || ldy < 12 || plane < 4LL * T * H * W) return YB_ERR_ARG;
   unpatchify2_clamp_kernel<<<grid_for(12LL * T * H * W), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
-      static_cast<const float*>(y), ldy, static_cast<float*>(out), T, H, W);
+      static_cast<const float*>(y), ldy, static_cast<float*>(out), T, H, W, plane);
   return check_launch("vae_unpatchify2_clamp");
+}
+
+extern "C" int yb_vae_unpatchify2_clamp(const void* y, long long ldy, void* out, int T, int H, int W, void* stream_) {
+  return yb_vae_unpatchify2_clamp_win(y, ldy, out, 4LL * T * H * W, T, H, W, stream_);
+}
+
+extern "C" int yb_nhwc_to_nchw_f32_clamp_win(const void* x, long long ldx, void* out, long long plane, long long N, int Cn,
+                                             float lo, float hi, void* stream_) {
+  if (!x || !out || N <= 0 || Cn <= 0 || ldx < Cn || plane < N || !(lo <= hi)) return YB_ERR_ARG;
+  nhwc_to_nchw_kernel<<<grid_for(N * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, lo, hi, plane);
+  return check_launch("nhwc_to_nchw_clamp");
 }

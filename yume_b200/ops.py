@@ -417,27 +417,51 @@ def conv3d_causal(xpad: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tens
     oob_zero_pad the input is the unpadded [T, H, W, Cp] and the zero padding is TMA out-of-bounds fill (Wan2.2 VAE).
     w bf16 [Cout, kt*kh*kw*Cp]; out rows are output voxels (frame t -> t*out_t_mul + out_t_add). stride_hw / stride_t = 2:
     the Encoder3d Resample convs (see include/yume_b200.h); T, H, W stay the input extents."""
-    global _launches, _flops
+    kt, kh, kw = taps
+    want = (T, H, W) if oob_zero_pad else (T + kt - 1, H + kh - 1, W + kw - 1)
+    args = _conv_args(xpad, w, bias, out, want, T, H, W, epilogue, res, taps, oob_zero_pad, out_t_mul, out_t_add, fuse_w,
+                      cta_pair, stride_t, stride_hw)
+    check(_lib.load().yb_conv3d_causal(C.byref(args), _stream()), "yb_conv3d_causal")
+    _count_conv(T, H, W, taps, stride_t, stride_hw, xpad.shape[-1], w.shape[0])
+    return out
+
+
+def conv3d_causal_hist(xbuf: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, T: int, H: int,
+                       W: int, t_hist: int, epilogue: int = YB_EPI_BF16, res: Optional[torch.Tensor] = None, taps=(3, 3, 3),
+                       out_t_mul: int = 1, out_t_add: int = 0, stride_t: int = 1, stride_hw: int = 1) -> torch.Tensor:
+    """History form of the zero-padded conv (include/yume_b200_stream.h): xbuf bf16 [t_hist + T, H, W, Cp] holds the t_hist
+    carried frames of the previous chunk in front of the T new ones (t_hist = kt - 1, or 1 for stride_t = 2)."""
+    args = _conv_args(xbuf, w, bias, out, (t_hist + T, H, W), T, H, W, epilogue, res, taps, True, out_t_mul, out_t_add, 0,
+                      None, stride_t, stride_hw)
+    check(_lib.load().yb_conv3d_causal_hist(C.byref(args), t_hist, _stream()), "yb_conv3d_causal_hist")
+    _count_conv(t_hist + T if stride_t > 1 else T, H, W, taps, stride_t, stride_hw, xbuf.shape[-1], w.shape[0])
+    return out
+
+
+def _conv_args(xpad, w, bias, out, want, T, H, W, epilogue, res, taps, oob_zero_pad, out_t_mul, out_t_add, fuse_w, cta_pair,
+               stride_t, stride_hw) -> Conv3dArgs:
     _need(xpad, torch.bfloat16, "xpad")
     _need(w, torch.bfloat16, "w")
     Cp = xpad.shape[-1]
     kt, kh, kw = taps
-    want = (T, H, W) if oob_zero_pad else (T + kt - 1, H + kh - 1, W + kw - 1)
-    if tuple(xpad.shape[:3]) != want or not xpad.is_contiguous() or w.shape[1] != kt * kh * kw * Cp or not w.is_contiguous():
+    if tuple(xpad.shape[:3]) != tuple(want) or not xpad.is_contiguous() or w.shape[1] != kt * kh * kw * Cp or \
+            not w.is_contiguous():
         raise YumeB200Error("conv3d_causal: bad input / weight layout")
     _need(out, torch.float32 if epilogue == YB_EPI_F32 else torch.bfloat16, "out")
     if res is not None:
         _need(res, torch.bfloat16, "res")
-    args = Conv3dArgs(struct_bytes=C.sizeof(Conv3dArgs), cta_pair=CONV_CTA_PAIR if cta_pair is None else cta_pair,
+    return Conv3dArgs(struct_bytes=C.sizeof(Conv3dArgs), cta_pair=CONV_CTA_PAIR if cta_pair is None else cta_pair,
                       xpad=xpad.data_ptr(), w=w.data_ptr(), bias=_ptr(bias), out=out.data_ptr(), res=_ptr(res),
                       ldo=out.stride(0), res_ld=(res.stride(0) if res is not None else 0), T=T, H=H, W=W, Cp=Cp,
                       Cout=w.shape[0], epilogue=epilogue, kt=kt, kh=kh, kw=kw, oob_zero_pad=1 if oob_zero_pad else 0,
                       out_t_mul=out_t_mul, out_t_add=out_t_add, fuse_w=fuse_w, stride_t=stride_t, stride_hw=stride_hw)
-    check(_lib.load().yb_conv3d_causal(C.byref(args), _stream()), "yb_conv3d_causal")
+
+
+def _count_conv(T, H, W, taps, stride_t, stride_hw, Cp, Cout) -> None:
+    global _launches, _flops
     _launches += 1
     To, Ho, Wo = conv_out_dims(T, H, W, taps, stride_t, stride_hw)
-    _flops += 2.0 * To * Ho * Wo * kt * kh * kw * Cp * w.shape[0]
-    return out
+    _flops += 2.0 * To * Ho * Wo * taps[0] * taps[1] * taps[2] * Cp * Cout
 
 
 def conv_out_dims(T: int, H: int, W: int, taps=(3, 3, 3), stride_t: int = 1, stride_hw: int = 1):
@@ -662,6 +686,82 @@ def vae_dupup_add(main: torch.Tensor, x: torch.Tensor, dims, in_c: int, out_c: i
                                        _stream()), "yb_vae_dupup_add")
     _launches += 1
     return main
+
+
+def vae_dupup_add_cont(main: torch.Tensor, x: torch.Tensor, dims, in_c: int, out_c: int, ft: int, fs: int) -> torch.Tensor:
+    """vae_dupup_add for a chunk after the first: main bf16 [ft*Ts, Hs*fs, Ws*fs, out_c], no duplicated frame dropped."""
+    global _launches
+    _need(main, torch.bfloat16, "main")
+    _need(x, torch.bfloat16, "x")
+    if not (main.is_contiguous() and x.is_contiguous()):
+        raise YumeB200Error("vae_dupup_add_cont needs dense tensors")
+    check(_lib.load().yb_vae_dupup_add_cont(main.data_ptr(), x.data_ptr(), dims[0], dims[1], dims[2], in_c, out_c, ft, fs,
+                                            _stream()), "yb_vae_dupup_add_cont")
+    _launches += 1
+    return main
+
+
+def _frame_window(out: torch.Tensor, Cn: int, T: int, name: str) -> int:
+    """Plane stride of out = video[:, t0:t0 + T] (f32 [Cn, T, h, w] view of a contiguous [Cn, T_all, h, w])."""
+    _need(out, torch.float32, name)
+    c, t, h, w = out.shape
+    if c != Cn or t != T or out.stride(3) != 1 or out.stride(2) != w or out.stride(1) != h * w:
+        raise YumeB200Error(f"{name}: out must be a frame window [{Cn}, {T}, h, w] of a contiguous video")
+    return out.stride(0)
+
+
+def vae_unpatchify2_clamp_win(y: torch.Tensor, out: torch.Tensor, T: int, H: int, W: int) -> torch.Tensor:
+    """vae_unpatchify2_clamp into out = video[:, t0:t0 + T] (f32 [3, T, 2H, 2W] frame window of the whole video)."""
+    global _launches
+    _need(y, torch.float32, "y")
+    plane = _frame_window(out, 3, T, "vae_unpatchify2_clamp_win")
+    check(_lib.load().yb_vae_unpatchify2_clamp_win(y.data_ptr(), y.stride(0), out.data_ptr(), plane, T, H, W, _stream()),
+          "yb_vae_unpatchify2_clamp_win")
+    _launches += 1
+    return out
+
+
+def nhwc_to_nchw_f32_win(x: torch.Tensor, out: torch.Tensor, clamp: Optional[tuple] = None) -> torch.Tensor:
+    """nhwc_to_nchw_f32 (optionally clamped) into out = video[:, t0:t0 + T] (f32 [Cn, T, h, w] frame window); x f32 [T*h*w, ldx]."""
+    global _launches
+    _need(x, torch.float32, "x")
+    Cn, T, h, w = out.shape
+    plane = _frame_window(out, Cn, T, "nhwc_to_nchw_f32_win")
+    if x.shape[0] != T * h * w:
+        raise YumeB200Error("nhwc_to_nchw_f32_win: x rows must be the window's voxels")
+    lo, hi = (-math.inf, math.inf) if clamp is None else clamp
+    check(_lib.load().yb_nhwc_to_nchw_f32_clamp_win(x.data_ptr(), x.stride(0), out.data_ptr(), plane, x.shape[0], Cn,
+                                                    float(lo), float(hi), _stream()), "yb_nhwc_to_nchw_f32_clamp_win")
+    _launches += 1
+    return out
+
+
+def vae_patchify2_bf16_win(video: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """vae_patchify2_bf16 from video = whole[:, t0:t0 + T] (f32 [3, T, H, W] frame window of a contiguous video)."""
+    global _launches
+    _, T, H, W = video.shape
+    plane = _frame_window(video, 3, T, "vae_patchify2_bf16_win")
+    _need(out, torch.bfloat16, "out")
+    if not out.is_contiguous():
+        raise YumeB200Error("vae_patchify2_bf16_win: out must be contiguous")
+    check(_lib.load().yb_vae_patchify2_bf16_win(video.data_ptr(), plane, out.data_ptr(), out.shape[-1], T, H, W, _stream()),
+          "yb_vae_patchify2_bf16_win")
+    _launches += 1
+    return out
+
+
+def nchw_to_nhwc_bf16_win(x: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """nchw_to_nhwc_bf16 from x = whole[:, t0:t0 + T] (f32 [Cn, T, H, W] frame window) into out bf16 [T*H*W, ldo]."""
+    global _launches
+    Cn, T, H, W = x.shape
+    plane = _frame_window(x, Cn, T, "nchw_to_nhwc_bf16_win")
+    _need(out, torch.bfloat16, "out")
+    if not out.is_contiguous() or out.shape[0] != T * H * W:
+        raise YumeB200Error("nchw_to_nhwc_bf16_win: out must be a contiguous [T*H*W, ldo]")
+    check(_lib.load().yb_nchw_to_nhwc_bf16_win(x.data_ptr(), plane, out.data_ptr(), out.shape[0], Cn, out.shape[1], _stream()),
+          "yb_nchw_to_nhwc_bf16_win")
+    _launches += 1
+    return out
 
 
 def vae_avgdown_add(main: torch.Tensor, x: torch.Tensor, dims, in_c: int, out_c: int, ft: int, fs: int) -> torch.Tensor:

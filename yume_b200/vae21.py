@@ -16,8 +16,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import ops
-from ._lib import YumeB200Error
-from .vae22 import _BF16, _F32, Wan22VaeDecoder
+from .vae22 import _F32, Wan22VaeDecoder
 
 Tensor = torch.Tensor
 
@@ -89,20 +88,15 @@ class Wan21VaeDecoder(Wan22VaeDecoder):
         std = torch.ones(z_dim) if std is None else std
         self._repack(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32))
 
-    @torch.no_grad()
-    def decode(self, z: Tensor) -> Tensor:
-        """z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 8H, 8W] clamped to [-1, 1] (WanVAE.decode :655-663)."""
-        if z.dim() != 4 or z.shape[0] != self.z_dim:
-            raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
-        zd, T, H, W = z.shape
-        N = T * H * W
-        zl = self._new(N, 64)
-        ops.nchw_to_nhwc_bf16(z.to(self.device, _F32).reshape(zd, N).contiguous(), zl)
-        w2, b2 = self.lin["conv2"]
-        x0 = torch.zeros(N, 64, device=self.device, dtype=_BF16)
-        ops.gemm(zl, w2, b2, x0[:, :w2.shape[0]], ops.YB_EPI_BF16)
-        dims = (T, H, W)
-        x = self._conv("decoder.conv1", x0.view(T, H, W, 64), dims)
+    def _t_ups(self) -> int:
+        return sum(1 for _, kind, _, _ in self.plan if kind == "upsample3d")
+
+    def _out_shape(self, T: int, H: int, W: int):
+        return 3, 1 + (T - 1) * (1 << self._t_ups()), 8 * H, 8 * W
+
+    def _decode_chunk(self, z: Tensor, out: Tensor) -> None:
+        """One chunk of `decode` (WanVAE.decode :655-663) into `out`, its frame window of the video."""
+        x, dims = self._front(z)
         x = self._res_block("decoder.middle.0", x, dims)
         x = self._attention("decoder.middle.1", x, dims)
         x = self._res_block("decoder.middle.2", x, dims)
@@ -112,10 +106,25 @@ class Wan21VaeDecoder(Wan22VaeDecoder):
                 x = self._res_block(p, x, dims)
             else:
                 x, dims = self._resample(p, x, dims, kind == "upsample3d")
-        y = self._conv("decoder.head.2", self._act(x, dims, "decoder.head.0", True), dims, epilogue=ops.YB_EPI_F32)
-        out = self._new(3, *dims, dtype=_F32)
-        ops.nhwc_to_nchw_f32(y, out.view(3, -1), clamp=(-1.0, 1.0))
-        return out
+        y = self._head(x, dims)
+        if self._chunk == 0 and not self._more:
+            ops.nhwc_to_nchw_f32(y, out.view(3, -1), clamp=(-1.0, 1.0))
+        else:
+            ops.nhwc_to_nchw_f32_win(y, out, (-1.0, 1.0))
+
+    def _level_plan(self, H: int, W: int) -> List[tuple]:
+        d0 = self.dims[0]
+        plan: List[tuple] = [("in", 1, H, W, 64, d0), ("res", 1, H, W, d0, d0), ("attn", 1, H, W, d0, 0), ("res", 1, H, W, d0, d0)]
+        s, h, w, last = 1, H, W, d0
+        for _, kind, ci, co in self.plan:
+            if kind == "res":
+                plan.append(("res", s, h, w, ci, co))
+            else:                                                # Resample's Conv2d halves the channels (:76-83)
+                plan.append(("up", s, h, w, ci, co, kind == "upsample3d", 0))
+                s, h, w = (2 * s if kind == "upsample3d" else s), 2 * h, 2 * w
+            last = co
+        plan.append(("head", s, h, w, last, self.conv["decoder.head.2"][0].shape[0]))
+        return plan
 
 
 def install_wan21_vae(vae, device="cuda"):

@@ -7,9 +7,12 @@ loop of T iterations, each launching the whole decoder on a single frame.
 
 H100 redesign: unrolling the cache logic shows every conv is a causal convolution over the whole frame sequence with
 zero padding in front (frame 0 skips `time_conv`, `time_conv` never sees frame 0, `DupUp3D` drops its first
-factor_t-1 frames — oracle/wan22vae.py states this and is pinned to the reference's chunked output). The decode is
-therefore ONE pass over [T, H, W, C] channels-last bf16 tensors; the whole sequence must fit in device memory (on an 80 GB H100
-a 49-frame 704x1280 chunk does, the 81-frame video does not):
+factor_t-1 frames — oracle/wan22vae.py states this and is pinned to the reference's chunked output). A decode is therefore a
+pass over [T, H, W, C] channels-last bf16 tensors of as many latent frames as fit in device memory (on an 80 GB H100 a 49-frame
+704x1280 video fits in one pass, the 81-frame video does not): `decode` splits the latent into chunks the planner sizes from the
+free device memory (one chunk whenever the whole sequence fits) and carries the reference's cache state from chunk to chunk —
+the last 2 input frames of every 3-tap causal conv, `time_conv`'s input stream from frame 1 on, DupUp3D's first-chunk drop —
+so every partition gives the one-pass result. Inside a chunk:
   * every conv (3x3x3, Conv2d 3x3 = (1,3,3), time_conv = (3,1,1)) is the wgmma implicit GEMM `yb_conv3d_causal` with
     `oob_zero_pad`: the causal zero padding is TMA out-of-bounds fill on the UNPADDED activation — no padded copy, no
     feature cache, no per-frame launches;
@@ -77,6 +80,11 @@ def decoder_param_shapes(dec_dim: int = 256, z_dim: int = 48, dim_mult: Sequence
 
 
 class Wan22VaeDecoder:
+    # chunk-streaming state of the running decode: chunk index, whether another chunk follows, carried conv input frames
+    _chunk, _more, _carry = 0, False, None
+    HIST = 2                     # carried frames of a 3-tap causal conv (the reference's CACHE_T)
+    MEM_MARGIN = 2 << 30         # bytes of free device memory the chunk planner leaves unused
+
     def __init__(self, sd: Dict[str, Tensor], dec_dim: int = 256, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_upsample: Sequence[bool] = (True, True, False),
                  mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
@@ -161,35 +169,67 @@ class Wan22VaeDecoder:
     def _new(self, *shape, dtype=_BF16) -> Tensor:
         return torch.empty(*shape, device=self.device, dtype=dtype)
 
+    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0) -> Tensor:
+        """Input buffer [h + T, H, W, Cp] of a conv whose input stream is `key`: after the first chunk its first h frames (n, or
+        HIST when n is 0) are the frames carried from the previous chunk and the producer writes the T new frames behind them."""
+        h = (n or self.HIST) if (key is not None and self._chunk > 0) else 0
+        buf = torch.zeros(h + T, H, W, Cp, device=self.device, dtype=_BF16) if zero else self._new(h + T, H, W, Cp)
+        if h:
+            buf[:h].copy_(self._carry[key])
+        return buf
+
+    def _keep(self, key: str, frames: Tensor, n: int = 0) -> None:
+        """Carry the last n (0: HIST) frames of the input stream `key` into the next chunk (zero frames in front where the stream
+        is shorter: the causal zero padding)."""
+        if not self._more:
+            return
+        n = n or self.HIST
+        if frames.shape[0] >= n:
+            self._carry[key] = frames[frames.shape[0] - n:].clone()
+        else:
+            c = torch.zeros(n, *frames.shape[1:], device=self.device, dtype=_BF16)
+            c[n - frames.shape[0]:].copy_(frames)
+            self._carry[key] = c
+
     def _conv(self, name: str, a: Tensor, dims, epilogue=None, res: Optional[Tensor] = None, out: Optional[Tensor] = None,
-              out_t_mul: int = 1, out_t_add: int = 0, stride_t: int = 1, stride_hw: int = 1) -> Tensor:
-        """a bf16 [T, H, W, Cp] (unpadded, dense) -> [To*Ho*Wo (or interleaved frames), cop]."""
+              out_t_mul: int = 1, out_t_add: int = 0, stride_t: int = 1, stride_hw: int = 1, key: Optional[str] = None) -> Tensor:
+        """a bf16 [h + T, H, W, Cp] (unpadded, dense; h carried frames in front, see _hist_buf) -> [To*Ho*Wo (or interleaved
+        frames), cop]. `key`: the input stream whose last frames the next chunk needs."""
         w, b, taps = self.conv[name]
         T, H, W = dims
+        h = a.shape[0] - T
+        if key is not None:                                      # a stride-2 time_conv carries one frame (vae2_2.py:158-170)
+            self._keep(key, a, 1 if stride_t > 1 else self.HIST)
         if epilogue is None:
             epilogue = ops.YB_EPI_RES_BF16 if res is not None else ops.YB_EPI_BF16
         if out is None:
             To, Ho, Wo = ops.conv_out_dims(T, H, W, taps, stride_t, stride_hw)
             out = self._new(To * Ho * Wo, w.shape[0], dtype=_F32 if epilogue == ops.YB_EPI_F32 else _BF16)
-        ops.conv3d_causal(a, w, b, out, T, H, W, epilogue, res, taps=taps, oob_zero_pad=True, out_t_mul=out_t_mul,
-                          out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
+        if h:
+            ops.conv3d_causal_hist(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, out_t_mul=out_t_mul,
+                                   out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
+        else:
+            ops.conv3d_causal(a, w, b, out, T, H, W, epilogue, res, taps=taps, oob_zero_pad=True, out_t_mul=out_t_mul,
+                              out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
         return out
 
-    def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1) -> Tensor:
+    def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1, key: Optional[str] = None,
+             n: int = 0) -> Tensor:
         T, H, W = dims
-        out = self._new(T, H * up, W * up, _rup(x.shape[1], 64))
-        ops.vae_rms_act(x, dims, out, self.gamma[gamma] if gamma else None, up, silu)
+        out = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n)
+        ops.vae_rms_act(x, dims, out[out.shape[0] - T:], self.gamma[gamma] if gamma else None, up, silu)
         return out
 
     def _res_block(self, p: str, x: Tensor, dims) -> Tensor:
         """ResidualBlock (:195-239)."""
-        y = self._conv(p + ".residual.2", self._act(x, dims, p + ".residual.0", True), dims)
+        c1, c2 = p + ".residual.2", p + ".residual.6"
+        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1), dims, key=c1)
         res = x
         if (p + ".shortcut") in self.lin:
             w, b = self.lin[p + ".shortcut"]
             res = self._new(x.shape[0], w.shape[0])
             ops.gemm(x, w, b, res, ops.YB_EPI_BF16)
-        return self._conv(p + ".residual.6", self._act(y, dims, p + ".residual.3", True), dims, res=res)
+        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2), dims, res=res, key=c2)
 
     def _attention(self, p: str, x: Tensor, dims) -> Tensor:
         """AttentionBlock (:242-283): per-frame single-head attention over H*W tokens, d = C."""
@@ -232,17 +272,33 @@ class Wan22VaeDecoder:
         return out
 
     def _resample(self, p: str, x: Tensor, dims, t_up: bool):
-        """Resample upsample2d / upsample3d (:73-170) over the whole sequence."""
+        """Resample upsample2d / upsample3d (:73-170) over the frames of this chunk."""
         T, H, W = dims
         N, C = x.shape
         HW = H * W
-        if t_up and T > 1:
-            xin = x[HW:].view(T - 1, H, W, C) if C % 64 == 0 else self._act(x[HW:], (T - 1, H, W), None, False)
-            y = self._new((2 * T - 1) * HW, C)
-            y[:HW].copy_(x[:HW])                                 # frame 0 bypasses time_conv ("Rep", :118-121)
-            for g in (0, 1):                                     # group g of input frame t -> output frame 1 + 2(t-1) + g
-                self._conv(f"{p}.time_conv.{g}", xin, (T - 1, H, W), out=y, out_t_mul=2, out_t_add=1 + g)
-            x, T = y, 2 * T - 1
+        if t_up:
+            # time_conv's input stream is every frame but frame 0, which bypasses it ("Rep", :118-121): in the first chunk it
+            # starts at the chunk's frame 1 (and may be empty), later chunks feed all their frames behind the carried history
+            first, key = self._chunk == 0, p + ".time_conv"
+            Ts = T - 1 if first else T
+            if Ts > 0:
+                src = x[HW:] if first else x
+                if C % 64:
+                    xin = self._act(src, (Ts, H, W), None, False, key=key)
+                elif first:
+                    xin = src.view(Ts, H, W, C)
+                else:
+                    xin = self._hist_buf(key, Ts, H, W, C)
+                    xin[self.HIST:].view(Ts * HW, C).copy_(src)
+                y = self._new((2 * Ts + (1 if first else 0)) * HW, C)
+                if first:
+                    y[:HW].copy_(x[:HW])
+                for g in (0, 1):                                 # group g of stream frame t -> output frame 2t + g (+1 after frame 0)
+                    self._conv(f"{p}.time_conv.{g}", xin, (Ts, H, W), out=y, out_t_mul=2, out_t_add=(1 if first else 0) + g,
+                               key=key if g == 0 else None)
+                x, T = y, y.shape[0] // HW
+            else:
+                self._keep(key, self._new(0, H, W, _rup(C, 64)))
         a = self._act(x, (T, H, W), None, False, up=2)           # nearest-exact 2x, then Conv2d 3x3 (zero pad 1)
         return self._conv(p + ".resample.1", a, (T, 2 * H, 2 * W)), (T, 2 * H, 2 * W)
 
@@ -256,32 +312,166 @@ class Wan22VaeDecoder:
             x = self._res_block(f"{p}.{j}", x, dims)
         if up_flag:
             x, dims = self._resample(f"{p}.{self.nrb + 1}", x, dims, t_up)
-            ops.vae_dupup_add(x, x_in, dims_in, ci, co, 2 if t_up else 1, 2)
+            dupup = ops.vae_dupup_add if self._chunk == 0 else ops.vae_dupup_add_cont     # DupUp3D `first_chunk` (:495-503)
+            dupup(x, x_in, dims_in, ci, co, 2 if t_up else 1, 2)
         return x, dims
 
-    @torch.no_grad()
-    def decode(self, z: Tensor) -> Tensor:
-        """z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 16H, 16W] clamped to [-1, 1] (Wan2_2_VAE.decode :1059-1072)."""
-        if z.dim() != 4 or z.shape[0] != self.z_dim:
-            raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
+    # ---- chunk streaming -----------------------------------------------------------------------------------
+    def _t_ups(self) -> int:
+        return sum(1 for i in range(self.n_up - 1) if i < len(self.t_up) and self.t_up[i])
+
+    def _front(self, z: Tensor):
+        """conv2 (latent de-normalisation folded in) and decoder.conv1 on one chunk of the latent."""
         zd, T, H, W = z.shape
         N = T * H * W
         zl = self._new(N, 64)
         ops.nchw_to_nhwc_bf16(z.to(self.device, _F32).reshape(zd, N).contiguous(), zl)
         w2, b2 = self.lin["conv2"]
-        x0 = torch.zeros(N, 64, device=self.device, dtype=_BF16)
-        ops.gemm(zl, w2, b2, x0[:, :w2.shape[0]], ops.YB_EPI_BF16)
+        x0 = self._hist_buf("decoder.conv1", T, H, W, 64, zero=True)
+        ops.gemm(zl, w2, b2, x0.view(-1, 64)[x0.shape[0] * H * W - N:, :w2.shape[0]], ops.YB_EPI_BF16)
         dims = (T, H, W)
-        x = self._conv("decoder.conv1", x0.view(T, H, W, 64), dims)
+        return self._conv("decoder.conv1", x0, dims, key="decoder.conv1"), dims
+
+    def _head(self, x: Tensor, dims) -> Tensor:
+        return self._conv("decoder.head.2", self._act(x, dims, "decoder.head.0", True, key="decoder.head.2"), dims,
+                          epilogue=ops.YB_EPI_F32, key="decoder.head.2")
+
+    def _decode_chunk(self, z: Tensor, out: Tensor) -> None:
+        """Decode one chunk of the latent into `out`, its frame window of the video."""
+        x, dims = self._front(z)
         x = self._res_block("decoder.middle.0", x, dims)
         x = self._attention("decoder.middle.1", x, dims)
         x = self._res_block("decoder.middle.2", x, dims)
         for i in range(self.n_up):
             x, dims = self._up_block(i, x, dims)
-        y = self._conv("decoder.head.2", self._act(x, dims, "decoder.head.0", True), dims, epilogue=ops.YB_EPI_F32)
-        out = self._new(3, dims[0], 2 * dims[1], 2 * dims[2], dtype=_F32)
-        ops.vae_unpatchify2_clamp(y, out, *dims)
+        y = self._head(x, dims)
+        if self._chunk == 0 and not self._more:
+            ops.vae_unpatchify2_clamp(y, out, *dims)
+        else:
+            ops.vae_unpatchify2_clamp_win(y, out, *dims)
+
+    def _out_shape(self, T: int, H: int, W: int) -> Tuple[int, int, int, int]:
+        s = 16                                                   # three 2x spatial upsamples, then unpatchify 2x
+        return 3, 1 + (T - 1) * (1 << self._t_ups()), s * H, s * W
+
+    @torch.no_grad()
+    def decode(self, z: Tensor) -> Tensor:
+        """z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 16H, 16W] clamped to [-1, 1] (Wan2_2_VAE.decode :1059-1072), in the chunks
+        `plan_chunks` sizes from the free device memory."""
+        if z.dim() != 4 or z.shape[0] != self.z_dim:
+            raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
+        return self._decode_chunks(z, self.plan_chunks(*z.shape[1:]))
+
+    def _decode_chunks(self, z: Tensor, lengths: Sequence[int]) -> Tensor:
+        """Decode the latent in chunks of `lengths` latent frames (any partition of T) into one preallocated video."""
+        T, H, W = z.shape[1:]
+        if sum(lengths) != T or min(lengths) < 1:
+            raise YumeB200Error(f"chunk lengths {list(lengths)} do not partition {T} latent frames")
+        out = self._new(*self._out_shape(T, H, W), dtype=_F32)
+        s = 1 << self._t_ups()
+        t0, f0 = 0, 0
+        self._carry = {}
+        try:
+            for i, n in enumerate(lengths):
+                self._chunk, self._more = i, i < len(lengths) - 1
+                nf = 1 + (n - 1) * s if i == 0 else n * s
+                self._decode_chunk(z[:, t0:t0 + n], out[:, f0:f0 + nf])
+                t0, f0 = t0 + n, f0 + nf
+        finally:
+            self._chunk, self._more, self._carry = 0, False, None
         return out
+
+    # ---- chunk planner -------------------------------------------------------------------------------------
+    def _level_plan(self, H: int, W: int) -> List[tuple]:
+        """The decoder's layer plan at latent size H x W, frames per chunk frame t_scale: ("in", t_scale, h, w, 64, co),
+        ("res", t_scale, h, w, ci, co), ("attn", t_scale, h, w, c, 0), ("up", t_scale, h, w, c, co_of_resample, temporal,
+        dupup_in) and ("head", t_scale, h, w, c, f32 output channels)."""
+        plan: List[tuple] = [("in", 1, H, W, 64, self.dims[0]), ("res", 1, H, W, self.dims[0], self.dims[0]),
+                             ("attn", 1, H, W, self.dims[0], 0), ("res", 1, H, W, self.dims[0], self.dims[0])]
+        s, h, w = 1, H, W
+        for i in range(self.n_up):
+            ci, co = self.dims[i], self.dims[i + 1]
+            for j in range(self.nrb + 1):
+                plan.append(("res", s, h, w, ci if j == 0 else co, co))
+            if i != self.n_up - 1:
+                t_up = i < len(self.t_up) and self.t_up[i]
+                plan.append(("up", s, h, w, co, co, t_up, ci))
+                s, h, w = (2 * s if t_up else s), 2 * h, 2 * w
+        plan.append(("head", s, h, w, self.dims[-1], self.conv["decoder.head.2"][0].shape[0]))
+        return plan
+
+    def _fixed_bytes(self, T: int, H: int, W: int) -> int:
+        """The whole result, allocated once before the first chunk."""
+        total = 1
+        for d in self._out_shape(T, H, W):
+            total *= d
+        return 4 * total
+
+    def chunk_bytes(self, n: int, T: int, H: int, W: int) -> int:
+        """Upper bound of the device bytes a decode (encode) of T latent (video) frames at H x W allocates on top of the weights
+        and its input when its chunks hold n latent frames: the whole result, every carried history, and the largest set of
+        activations one step of the layer plan keeps live (every buffer of that step counted as live at once; a chunk after
+        the first is counted, it has the most frames at each level)."""
+        bf, f4 = 2, 4
+        hist = self.HIST
+        carries, peak = 0, 0
+        for step in self._level_plan(H, W):
+            kind, s, h, w, c = step[:5]
+            F, vox = n * s, h * w
+            cp = _rup(c, 64)
+            if kind == "in":                                     # input gather, conv1's input buffer (history in front), conv1 out
+                carries += hist * vox * c * bf
+                live = (F * vox * c + (F + hist) * vox * c + F * vox * step[5]) * bf
+            elif kind == "down":                                 # x, held block input, act, resample.1 out (+1 carried frame),
+                vq = (h // 2) * (w // 2)                         # its act, time_conv out
+                live = (F * vox * (c + step[6] + cp) + (F + 1) * vq * (c + cp) + F * vq * c) * bf
+                if step[5]:
+                    carries += vq * cp * bf
+            elif kind == "res":                                    # x, the block input a shortcut add holds, y, res, out, two acts
+                ci, co = c, step[5]
+                carries += hist * vox * (cp + _rup(co, 64)) * bf
+                live = F * vox * (2 * ci + 3 * co) * bf + (F + hist) * vox * (cp + _rup(co, 64)) * bf
+            elif kind == "attn":
+                Lf, Next = _rup(vox, 32), _rup(F * vox, 32) + 32
+                live = (F * vox * c * 5 + Next * c * 3 + F * Lf * c * 3) * bf + vox * Lf * (f4 + bf)
+            elif kind == "up":
+                co, t_up, dup_in = step[5], step[6], step[7]
+                F2 = 2 * F if t_up else F
+                live = (F * vox * (c + dup_in) + F2 * vox * c) * bf + (F + hist) * vox * cp * bf * (1 if t_up else 0)
+                live += F2 * 4 * vox * (cp + _rup(co, 32)) * bf
+                if t_up:
+                    carries += hist * vox * cp * bf
+            else:                                                # head: act, f32 conv output
+                live = (F * vox * c + (F + hist) * vox * cp) * bf + F * vox * step[5] * f4
+                carries += hist * vox * cp * bf
+            peak = max(peak, live)
+        return self._fixed_bytes(T, H, W) + carries + peak
+
+    def _plan(self, units: int, nbytes) -> List[int]:
+        """Latent frames per chunk: all `units` when they fit (and always off CUDA), else the longest chunks whose `nbytes`
+        fit the device's free memory (free + torch's cached, unallocated blocks) minus MEM_MARGIN. The free memory is read
+        when the call starts, so other work on the same GPU can make a sequence that would fit alone run in chunks (with the
+        same result)."""
+        if self.device.type != "cuda":
+            return [units]
+        free, _ = torch.cuda.mem_get_info(self.device)
+        free += torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+        return chunk_lengths(units, nbytes, free - self.MEM_MARGIN)
+
+    def plan_chunks(self, T: int, H: int, W: int) -> List[int]:
+        """Latent frames per chunk of a decode of a T-frame latent at H x W (see _plan)."""
+        return self._plan(T, lambda n: self.chunk_bytes(n, T, H, W))
+
+
+def chunk_lengths(T: int, nbytes, budget: int) -> List[int]:
+    """Partition T latent frames into chunks of the longest length n whose `nbytes(n)` (non-decreasing in n) fits `budget`, the
+    last chunk taking the remainder: [T] when the whole sequence fits, chunks of 1 frame when nothing longer does."""
+    if nbytes(T) <= budget:
+        return [T]
+    n = 1
+    while n + 1 < T and nbytes(n + 1) <= budget:
+        n += 1
+    return [n] * (T // n) + ([T % n] if T % n else [])
 
 
 def install_wan22_vae(vae, device="cuda"):

@@ -5,8 +5,11 @@ wan/image2video.py:348-367).
 Reference: /root/reference/wan23/modules/vae2_2.py `WanVAE_.encode` (:796-829) and /root/reference/wan/modules/vae.py (:515-542)
 encode frame 0 alone and then 4 frames per `Encoder3d.forward` call, threading a feature cache through every `CausalConv3d`.
 Unrolled (oracle/wan22vae_enc.py, oracle/wan21vae_enc.py, both pinned to the reference's chunked output) every conv is a causal
-conv over the whole frame sequence, so the H100 path is the decoder's design run backwards: ONE pass over channels-last bf16
-[T, H, W, C] tensors on the wgmma implicit-GEMM conv, with the two strided `Resample` convs done by the tensor map itself —
+conv over the whole frame sequence, so the H100 path is the decoder's design run backwards: a pass over channels-last bf16
+[T, H, W, C] tensors on the wgmma implicit-GEMM conv — one pass when the video fits in device memory, else chunks of 1 + 4a, then 4b
+frames carrying the reference's cache state (the decoder's 2-frame conv histories; the last input frame of the stride-2
+`time_conv`; AvgDown3D pads in front exactly where its per-call padding does, i.e. only in the first chunk) — with the two strided
+`Resample` convs done by the tensor map itself —
   * `Resample(downsample2d)`: ZeroPad2d((0,1,0,1)) + Conv2d(3x3, stride 2) (vae2_2.py:101-104) = `yb_conv3d_causal` with
     `stride_hw = 2`: TMA `elementStrides` sample every second voxel, the pad row/column behind the data is out-of-bounds fill;
   * `Resample(downsample3d)` (:105-110, :158-170): frame 0 bypasses `time_conv`, the rest is CausalConv3d((3,1,1),
@@ -14,12 +17,12 @@ conv over the whole frame sequence, so the H100 path is the decoder's design run
   * Wan2.2 only: the `AvgDown3D` shortcut of `Down_ResidualBlock` (:320-373, :449-459) is one gather-add, the input `patchify`
     (:284-300) one gather;
   * `conv1` (1x1x1) with the latent normalisation (mu - mean) / std folded into its weights; only the mu half is computed.
-No feature cache, no per-chunk launches, no padded or strided copy of any activation.
+No padded or strided copy of any activation.
 """
 from __future__ import annotations
 
 import types
-from typing import Dict, Optional, Sequence
+from typing import Dict, List, Optional, Sequence
 
 import torch
 
@@ -123,12 +126,22 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
 
     # ---- building blocks the decoder does not have -----------------------------------------------------------
     def _resample_down(self, p: str, x: Tensor, dims, temporal: bool):
-        """Resample downsample2d / downsample3d over the whole sequence (vae2_2.py:101-110, 152-170; vae.py:84-90, 125-139)."""
+        """Resample downsample2d / downsample3d over the frames of this chunk (vae2_2.py:101-110, 152-170; vae.py:84-90,
+        125-139). The stride-2 time_conv carries the last frame of its input to the next chunk; frame 0 passes only in the first."""
         T, H, W = dims
         C = x.shape[1]
         a = x.view(T, H, W, C) if C % 64 == 0 else self._act(x, dims, None, False)
-        y = self._conv(p + ".resample.1", a, dims, stride_hw=2)
         _, Ho, Wo = ops.conv_out_dims(T, H, W, (1, 3, 3), 1, 2)
+        key = p + ".time_conv"
+        if temporal and self._chunk > 0:
+            # resample.1 writes behind the carried frame; time_conv reads [carried, 2b new frames] -> b frames
+            ybuf = self._hist_buf(key, T, Ho, Wo, C, n=1) if C % 64 == 0 else None
+            y = self._conv(p + ".resample.1", a, dims, stride_hw=2, out=None if ybuf is None else ybuf[1:].view(-1, C))
+            ain = ybuf if ybuf is not None else self._act(y, (T, Ho, Wo), None, False, key=key, n=1)
+            z = self._new((T // 2) * Ho * Wo, C)
+            self._conv(p + ".time_conv", ain, (T, Ho, Wo), out=z, stride_t=2, key=key)
+            return z, (T // 2, Ho, Wo)
+        y = self._conv(p + ".resample.1", a, dims, stride_hw=2)
         if temporal and T > 1:
             if T < 3:
                 raise YumeB200Error("downsample3d needs 1 or >= 3 frames (the reference feeds 1 + 4k)")
@@ -136,8 +149,10 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
             To = (T - 3) // 2 + 1
             z = self._new((1 + To) * Ho * Wo, C)
             z[:Ho * Wo].copy_(y[:Ho * Wo])                         # frame 0 passes ("Rep" branch, :158-163)
-            self._conv(p + ".time_conv", a, (T, Ho, Wo), out=z, out_t_add=1, stride_t=2)
+            self._conv(p + ".time_conv", a, (T, Ho, Wo), out=z, out_t_add=1, stride_t=2, key=key)
             return z, (1 + To, Ho, Wo)
+        if temporal and self._more:                                # frame 0 alone: it is the next chunk's history
+            self._keep(key, y.view(T, Ho, Wo, C) if C % 64 == 0 else self._act(y, (T, Ho, Wo), None, False), 1)
         return y, (T, Ho, Wo)
 
     def _down_block(self, i: int, x: Tensor, dims):
@@ -159,33 +174,102 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
         keep = 1 + 4 * ((video.shape[1] - 1) // 4)                 # `iter_ = 1 + (t - 1) // 4` chunks of 1, 4, 4, ... (:802-803)
         return video[:, :keep].to(self.device, _F32).contiguous()
 
-    def _head(self, x: Tensor, dims) -> Tensor:
-        y = self._conv("encoder.head.2", self._act(x, dims, "encoder.head.0", True), dims)
+    def _head(self, x: Tensor, dims, out: Tensor) -> None:
+        """encoder.head + conv1 (mu half) into `out`, this chunk's latent-frame window of the result."""
+        k = "encoder.head.2"
+        y = self._conv(k, self._act(x, dims, "encoder.head.0", True, key=k), dims, key=k)
         w1, b1 = self.lin["conv1"]
         mu = self._new(y.shape[0], w1.shape[0], dtype=_F32)
         ops.gemm(y, w1, b1, mu, ops.YB_EPI_F32)
-        out = self._new(self.z_dim, *dims, dtype=_F32)
-        ops.nhwc_to_nchw_f32(mu, out.view(self.z_dim, -1))
-        return out
+        if self._chunk == 0 and not self._more:
+            ops.nhwc_to_nchw_f32(mu, out.view(self.z_dim, -1))
+        else:
+            ops.nhwc_to_nchw_f32_win(mu, out)
 
     def _middle(self, x: Tensor, dims) -> Tensor:
         x = self._res_block("encoder.middle.0", x, dims)
         x = self._attention("encoder.middle.1", x, dims)
         return self._res_block("encoder.middle.2", x, dims)
 
-    @torch.no_grad()
-    def encode(self, video: Tensor) -> Tensor:
-        video = self._frames(video)
-        _, T, H, W = video.shape
+    # ---- chunk streaming -----------------------------------------------------------------------------------
+    SCALE = 16                                                     # spatial downsampling of the latent
+
+    def _check_hw(self, H: int, W: int) -> None:
         if H % 16 or W % 16:
             raise YumeB200Error("Wan2.2 VAE encode needs H, W divisible by 16 (patchify 2 x three stride-2 levels)")
+
+    def _input(self, v: Tensor):
+        """encoder.conv1's input buffer (carried frames in front) with this chunk's patchified frames behind them."""
+        _, T, H, W = v.shape
         dims = (T, H // 2, W // 2)
-        x0 = self._new(dims[0] * dims[1] * dims[2], 64)
-        ops.vae_patchify2_bf16(video, x0)
-        x = self._conv("encoder.conv1", x0.view(*dims, 64), dims)
+        x0 = self._hist_buf("encoder.conv1", *dims, 64)
+        dst = x0[x0.shape[0] - T:].view(-1, 64)
+        if self._chunk == 0 and not self._more:
+            ops.vae_patchify2_bf16(v, dst)
+        else:
+            ops.vae_patchify2_bf16_win(v, dst)
+        return x0, dims
+
+    def _encode_chunk(self, v: Tensor, out: Tensor) -> None:
+        x0, dims = self._input(v)
+        x = self._conv("encoder.conv1", x0, dims, key="encoder.conv1")
         for i in range(self.n_down):
             x, dims = self._down_block(i, x, dims)
-        return self._head(self._middle(x, dims), dims)
+        self._head(self._middle(x, dims), dims, out)
+
+    @torch.no_grad()
+    def encode(self, video: Tensor) -> Tensor:
+        """video f32 [3, T, H, W] -> mu [z_dim, 1 + (T-1)//4, H/s, W/s], in the chunks `plan_chunks` sizes from the free device
+        memory."""
+        video = self._frames(video)
+        return self._encode_chunks(video, self.plan_chunks(*video.shape[1:]))
+
+    def _encode_chunks(self, video: Tensor, lengths: Sequence[int]) -> Tensor:
+        """Encode in chunks of `lengths` LATENT frames (a partition of 1 + (T-1)//4): the first chunk reads 1 + 4(n-1) video
+        frames, every later one 4n (the reference's frame 0, then 4 frames per call)."""
+        video = self._frames(video)
+        _, T, H, W = video.shape
+        self._check_hw(H, W)
+        Tl = 1 + (T - 1) // 4
+        if sum(lengths) != Tl or min(lengths) < 1:
+            raise YumeB200Error(f"chunk lengths {list(lengths)} do not partition {Tl} latent frames")
+        out = self._new(self.z_dim, Tl, H // self.SCALE, W // self.SCALE, dtype=_F32)
+        t0, f0 = 0, 0
+        self._carry = {}
+        try:
+            for i, n in enumerate(lengths):
+                self._chunk, self._more = i, i < len(lengths) - 1
+                nv = 1 + 4 * (n - 1) if i == 0 else 4 * n
+                self._encode_chunk(video[:, f0:f0 + nv], out[:, t0:t0 + n])
+                t0, f0 = t0 + n, f0 + nv
+        finally:
+            self._chunk, self._more, self._carry = 0, False, None
+        return out
+
+    def _fixed_bytes(self, T: int, H: int, W: int) -> int:
+        """mu, and the device copy of the video `encode` makes when it is handed one on another device or not contiguous."""
+        return 4 * (self.z_dim * (1 + (T - 1) // 4) * (H // self.SCALE) * (W // self.SCALE) + 3 * T * H * W)
+
+    def _level_plan(self, H: int, W: int) -> List[tuple]:
+        """The encoder's layer plan at video size H x W, frames per latent frame of a chunk first (see Wan22VaeDecoder)."""
+        d, s, h, w = self.dims, 4, H // 2, W // 2
+        plan: List[tuple] = [("in", s, h, w, 64, d[0])]
+        for i in range(self.n_down):
+            for j in range(self.nrb):
+                plan.append(("res", s, h, w, d[i] if j == 0 else d[i + 1], d[i + 1]))
+            if i != self.n_down - 1:
+                t = i < len(self.t_down) and self.t_down[i]
+                plan.append(("down", s, h, w, d[i + 1], t, d[i]))
+                s, h, w = (s // 2 if t else s), h // 2, w // 2
+        return plan + self._tail_plan(s, h, w, d[-1])
+
+    def _tail_plan(self, s: int, h: int, w: int, c: int) -> List[tuple]:
+        return [("res", s, h, w, c, c), ("attn", s, h, w, c, 0), ("res", s, h, w, c, c),
+                ("head", s, h, w, c, _rup(2 * self.z_dim, 32) + 2 * _rup(self.z_dim, 32))]
+
+    def plan_chunks(self, T: int, H: int, W: int) -> List[int]:
+        """Latent frames per chunk of an encode of T video frames at H x W (see Wan22VaeDecoder._plan)."""
+        return self._plan(1 + (T - 1) // 4, lambda n: self.chunk_bytes(n, T, H, W))
 
     def decode(self, z):                                           # the inherited decoder entry point has no weights here
         raise YumeB200Error("this engine holds the encoder side; use Wan22VaeDecoder for decode")
@@ -200,7 +284,7 @@ class Wan21VaeEncoder(Wan22VaeEncoder):
                  mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
         self.device = torch.device(device)
         self.z_dim = z_dim
-        dims = [dim * u for u in [1] + list(dim_mult)]
+        self.enc_dims = dims = [dim * u for u in [1] + list(dim_mult)]
         self.plan, n = [], 0
         for i in range(len(dim_mult)):
             for _ in range(num_res_blocks):
@@ -213,23 +297,46 @@ class Wan21VaeEncoder(Wan22VaeEncoder):
         std = torch.ones(z_dim) if std is None else std
         self._repack_encoder(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32), dims[-1])
 
-    @torch.no_grad()
-    def encode(self, video: Tensor) -> Tensor:
-        video = self._frames(video)
-        _, T, H, W = video.shape
+    SCALE = 8
+
+    def _check_hw(self, H: int, W: int) -> None:
         if H % 8 or W % 8:
             raise YumeB200Error("Wan2.1 VAE encode needs H, W divisible by 8")
-        dims = (T, H, W)
-        x0 = self._new(T * H * W, 64)
-        ops.nchw_to_nhwc_bf16(video.view(3, -1), x0)
-        x = self._conv("encoder.conv1", x0.view(T, H, W, 64), dims)
+
+    def _input(self, v: Tensor):
+        _, T, H, W = v.shape
+        x0 = self._hist_buf("encoder.conv1", T, H, W, 64)
+        dst = x0[x0.shape[0] - T:].view(-1, 64)
+        if self._chunk == 0 and not self._more:
+            ops.nchw_to_nhwc_bf16(v.view(3, -1), dst)
+        else:
+            ops.nchw_to_nhwc_bf16_win(v, dst)
+        return x0, (T, H, W)
+
+    def _encode_chunk(self, v: Tensor, out: Tensor) -> None:
+        x0, dims = self._input(v)
+        x = self._conv("encoder.conv1", x0, dims, key="encoder.conv1")
         for n, kind in self.plan:
             p = f"encoder.downsamples.{n}"
             if kind == "res":
                 x = self._res_block(p, x, dims)
             else:
                 x, dims = self._resample_down(p, x, dims, kind == "downsample3d")
-        return self._head(self._middle(x, dims), dims)
+        self._head(self._middle(x, dims), dims, out)
+
+    def _level_plan(self, H: int, W: int) -> List[tuple]:
+        d, s, h, w = self.enc_dims, 4, H, W
+        plan: List[tuple] = [("in", s, h, w, 64, d[0])]
+        level, c = 0, d[0]
+        for _, kind in self.plan:
+            if kind == "res":
+                plan.append(("res", s, h, w, c, d[level + 1]))
+                c = d[level + 1]
+            else:
+                t = kind == "downsample3d"
+                plan.append(("down", s, h, w, c, t, 0))
+                s, h, w, level = (s // 2 if t else s), h // 2, w // 2, level + 1
+        return plan + self._tail_plan(s, h, w, c)
 
 
 def install_wan22_vae_encoder(vae, device="cuda"):
