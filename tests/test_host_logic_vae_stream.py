@@ -22,7 +22,7 @@ import test_gpu_vae_stream as KS
 from helpers import torch_ops_stream
 from oracle import wan21vae, wan21vae_enc, wan22vae, wan22vae_enc
 from test_kernel_contract_cpu import _entry_problems
-from yume_b200 import vae21, vae22, vae_enc
+from yume_b200 import vae21, vae22, vae_enc, wan_vae
 
 STREAM_HEADER = Path(__file__).resolve().parents[1] / "include" / "yume_b200_stream.h"
 DEC_PARTS = [[1] * 9, [2, 7], [4, 5], [1, 3, 5], [8, 1], [3, 3, 3]]
@@ -118,9 +118,9 @@ def test_dropped_or_shifted_carries_are_detected(cpu_ops, gold, monkeypatch):
 @pytest.mark.parametrize("which", ["wan22", "wan21"])
 def test_one_chunk_decode_and_encode_issue_the_one_pass_launches(cpu_ops, gold, monkeypatch, which):
     kept = []
-    keep = vae22.Wan22VaeDecoder._keep
-    monkeypatch.setattr(vae22.Wan22VaeDecoder, "_keep", lambda self, key, f, n=0: (kept.append(key) if self._more else None,
-                                                                                    keep(self, key, f, n)))
+    keep = wan_vae.WanVaeEngine._keep                            # every engine's carries go through the base's _keep
+    monkeypatch.setattr(wan_vae.WanVaeEngine, "_keep", lambda self, key, f, n=0: (kept.append(key) if self._more else None,
+                                                                                 keep(self, key, f, n)))
     streaming = {"conv3d_causal_hist", "vae_dupup_add_cont", "vae_unpatchify2_clamp_win", "nhwc_to_nchw_f32_win",
                  "vae_patchify2_bf16_win", "nchw_to_nhwc_bf16_win"}
     eng, z, c = _decoder(gold, which)

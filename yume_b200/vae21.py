@@ -3,7 +3,7 @@ fastvideo/sample/sample.py). SURVEY.md §8(f) "next" row, rank 1 (second half).
 
 Reference: /root/reference/wan/modules/vae.py (≡ wan23/modules/vae2_1.py) — `WanVAE_.decode` (:544-568) decodes one
 latent frame per `Decoder3d.forward` call through a per-conv feature cache. As for the 2.2 VAE (yume_b200/vae22.py, whose
-building blocks this engine reuses) the cache logic unrolls to causal convs over the whole sequence, so the H100 path is a
+decode side this engine shares) the cache logic unrolls to causal convs over the whole sequence, so the H100 path is a
 single pass of wgmma implicit-GEMM convs with TMA zero fill as the padding. What differs from 2.2: the flat
 `decoder.upsamples` Sequential (:395-414), `Resample`'s Conv2d halves the channels (:76-83) so blocks 1..3 start at
 dims[i] // 2 (:398-399), there is no DupUp3D shortcut, and the head conv emits RGB directly (no unpatchify).
@@ -16,7 +16,8 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import torch
 
 from . import ops
-from .vae22 import _F32, Wan22VaeDecoder
+from .vae22 import WanVaeDecoder, decoder_front
+from .wan_vae import Layer, _rup
 
 Tensor = torch.Tensor
 
@@ -76,55 +77,27 @@ def decoder_param_shapes(dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int]
     return s
 
 
-class Wan21VaeDecoder(Wan22VaeDecoder):
+class Wan21VaeDecoder(WanVaeDecoder):
+    """`WanVAE.decode` (vae.py:655-663): z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 8H, 8W]."""
+    SCALE = 8
+
     def __init__(self, sd: Dict[str, Tensor], dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_upsample: Sequence[bool] = (True, True, False),
                  mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
-        self.device = torch.device(device)
-        self.z_dim = z_dim
-        self.dims = [dim * dim_mult[-1]]                         # attention width (decoder.middle.1)
         self.plan = upsample_plan(dim, dim_mult, num_res_blocks, temperal_upsample)
-        mean = torch.zeros(z_dim) if mean is None else mean
-        std = torch.ones(z_dim) if std is None else std
-        self._repack(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32))
-
-    def _t_ups(self) -> int:
-        return sum(1 for _, kind, _, _ in self.plan if kind == "upsample3d")
-
-    def _out_shape(self, T: int, H: int, W: int):
-        return 3, 1 + (T - 1) * (1 << self._t_ups()), 8 * H, 8 * W
-
-    def _decode_chunk(self, z: Tensor, out: Tensor) -> None:
-        """One chunk of `decode` (WanVAE.decode :655-663) into `out`, its frame window of the video."""
-        x, dims = self._front(z)
-        x = self._res_block("decoder.middle.0", x, dims)
-        x = self._attention("decoder.middle.1", x, dims)
-        x = self._res_block("decoder.middle.2", x, dims)
-        for n, kind, _, _ in self.plan:
+        layers = decoder_front(dim * dim_mult[-1])
+        for n, kind, ci, co in self.plan:                        # Resample's Conv2d halves the channels (:76-83)
             p = f"decoder.upsamples.{n}"
-            if kind == "res":
-                x = self._res_block(p, x, dims)
-            else:
-                x, dims = self._resample(p, x, dims, kind == "upsample3d")
-        y = self._head(x, dims)
-        if self._chunk == 0 and not self._more:
+            ft = 2 if kind == "upsample3d" else 1
+            layers.append(Layer("res", p, ci, co) if kind == "res" else Layer("up", p, ci, co, ft, 2))
+        layers.append(Layer("head", "decoder.head.2", self.plan[-1][3], _rup(3, 32)))
+        super().__init__(sd, z_dim, layers, mean, std, device)
+
+    def _write(self, y: Tensor, out: Tensor, dims) -> None:
+        if self._one_pass:
             ops.nhwc_to_nchw_f32(y, out.view(3, -1), clamp=(-1.0, 1.0))
         else:
             ops.nhwc_to_nchw_f32_win(y, out, (-1.0, 1.0))
-
-    def _level_plan(self, H: int, W: int) -> List[tuple]:
-        d0 = self.dims[0]
-        plan: List[tuple] = [("in", 1, H, W, 64, d0), ("res", 1, H, W, d0, d0), ("attn", 1, H, W, d0, 0), ("res", 1, H, W, d0, d0)]
-        s, h, w, last = 1, H, W, d0
-        for _, kind, ci, co in self.plan:
-            if kind == "res":
-                plan.append(("res", s, h, w, ci, co))
-            else:                                                # Resample's Conv2d halves the channels (:76-83)
-                plan.append(("up", s, h, w, ci, co, kind == "upsample3d", 0))
-                s, h, w = (2 * s if kind == "upsample3d" else s), 2 * h, 2 * w
-            last = co
-        plan.append(("head", s, h, w, last, self.conv["decoder.head.2"][0].shape[0]))
-        return plan
 
 
 def install_wan21_vae(vae, device="cuda"):

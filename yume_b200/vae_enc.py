@@ -5,7 +5,8 @@ wan/image2video.py:348-367).
 Reference: /root/reference/wan23/modules/vae2_2.py `WanVAE_.encode` (:796-829) and /root/reference/wan/modules/vae.py (:515-542)
 encode frame 0 alone and then 4 frames per `Encoder3d.forward` call, threading a feature cache through every `CausalConv3d`.
 Unrolled (oracle/wan22vae_enc.py, oracle/wan21vae_enc.py, both pinned to the reference's chunked output) every conv is a causal
-conv over the whole frame sequence, so the H100 path is the decoder's design run backwards: a pass over channels-last bf16
+conv over the whole frame sequence, so the H100 path is the decoder's design run backwards, on the building blocks of
+yume_b200/wan_vae.py: a pass over channels-last bf16
 [T, H, W, C] tensors on the wgmma implicit-GEMM conv — one pass when the video fits in device memory, else chunks of 1 + 4a, then 4b
 frames carrying the reference's cache state (the decoder's 2-frame conv histories; the last input frame of the stride-2
 `time_conv`; AvgDown3D pads in front exactly where its per-call padding does, i.e. only in the first chunk) — with the two strided
@@ -28,7 +29,7 @@ import torch
 
 from . import ops
 from ._lib import YumeB200Error
-from .vae22 import _BF16, _F32, Wan22VaeDecoder, _rup
+from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _rup
 
 Tensor = torch.Tensor
 
@@ -96,24 +97,25 @@ def encoder_param_shapes_21(dim: int = 96, z_dim: int = 16, dim_mult: Sequence[i
     return s
 
 
-class Wan22VaeEncoder(Wan22VaeDecoder):
-    """`Wan2_2_VAE.encode` for one video: f32 [3, T, H, W] -> mu f32 [z_dim, 1 + (T-1)//4, H/16, W/16]. The building blocks
-    (`_conv`, `_act`, `_res_block`, `_attention`) are the decoder's."""
+def _encoder_tail(c: int, z_dim: int) -> List[Layer]:
+    """encoder.middle and encoder.head (+ conv1's mu half): the last layers of both Wan encoders."""
+    return [Layer("res", "encoder.middle.0", c, c), Layer("attn", "encoder.middle.1", c), Layer("res", "encoder.middle.2", c, c),
+            Layer("head", "encoder.head.2", c, _rup(2 * z_dim, 32) + 2 * _rup(z_dim, 32))]
 
-    def __init__(self, sd: Dict[str, Tensor], dim: int = 160, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
-                 num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
-        self.device = torch.device(device)
-        self.z_dim, self.nrb = z_dim, num_res_blocks
-        self.dims = [dim * u for u in [1] + list(dim_mult)]                         # vae2_2.py:527
-        self.t_down, self.n_down = list(temperal_downsample), len(dim_mult)
-        mean = torch.zeros(z_dim) if mean is None else mean
-        std = torch.ones(z_dim) if std is None else std
-        self._repack_encoder(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32), self.dims[-1])
 
-    def _repack_encoder(self, sd: Dict[str, Tensor], mean: Tensor, std: Tensor, width: int) -> None:
+class WanVaeEncoder(WanVaeEngine):
+    """The encode side of both Wan VAEs: f32 [3, T, H, W] -> mu f32 [z_dim, 1 + (T-1)//4, H/SCALE, W/SCALE]. An engine adds its
+    layer list, SCALE and `_read` (the chunk's video frames into encoder.conv1's input)."""
+    SCALE: int
+
+    @property
+    def ops(self):
+        """This module's op library (see WanVaeEngine)."""
+        return ops
+
+    def _repack(self, sd: Dict[str, Tensor], mean: Tensor, std: Tensor) -> None:
         dev = self.device
-        sd = self._pack_side(sd, ("encoder.", "conv1."), "conv1", "encoder.middle.1", width, False)
+        sd = self._pack_side(sd, ("encoder.", "conv1."), "conv1", False)
         # conv1 (1x1x1, 2z -> 2z), mu half only (`.chunk(2, dim=1)[0]`, :822), normalisation folded in:
         # (W x + b - mean) / std = (diag(1/std) W) x + (b - mean) / std
         zd = self.z_dim
@@ -124,10 +126,18 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
         b[:zd] = (sd["conv1.bias"].detach().float()[:zd] - mean) / std
         self.lin["conv1"] = (w.to(dev, _BF16).contiguous(), b.to(dev))
 
-    # ---- building blocks the decoder does not have -----------------------------------------------------------
-    def _resample_down(self, p: str, x: Tensor, dims, temporal: bool):
+    def _input(self, L: Layer, v: Tensor):
+        """encoder.conv1 over its input buffer: carried frames in front, this chunk's frames (patch size L.fs) behind them."""
+        _, T, H, W = v.shape
+        dims = (T, H // L.fs, W // L.fs)
+        x0 = self._hist_buf(L.name, *dims, 64)
+        self._read(v, x0[x0.shape[0] - T:].view(-1, 64))
+        return self._conv(L.name, x0, dims, key=L.name), dims
+
+    def _resample(self, L: Layer, x: Tensor, dims):
         """Resample downsample2d / downsample3d over the frames of this chunk (vae2_2.py:101-110, 152-170; vae.py:84-90,
         125-139). The stride-2 time_conv carries the last frame of its input to the next chunk; frame 0 passes only in the first."""
+        p, temporal = L.name, L.ft == 2
         T, H, W = dims
         C = x.shape[1]
         a = x.view(T, H, W, C) if C % 64 == 0 else self._act(x, dims, None, False)
@@ -155,67 +165,22 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
             self._keep(key, y.view(T, Ho, Wo, C) if C % 64 == 0 else self._act(y, (T, Ho, Wo), None, False), 1)
         return y, (T, Ho, Wo)
 
-    def _down_block(self, i: int, x: Tensor, dims):
-        """Down_ResidualBlock (:420-459)."""
-        p = f"encoder.downsamples.{i}.downsamples"
-        down = i != self.n_down - 1
-        t_down = self.t_down[i] if i < len(self.t_down) else False
-        x_in, dims_in = x, dims
-        for j in range(self.nrb):
-            x = self._res_block(f"{p}.{j}", x, dims)
-        if down:
-            x, dims = self._resample_down(f"{p}.{self.nrb}", x, dims, t_down)
-        ops.vae_avgdown_add(x, x_in, dims_in, x_in.shape[1], x.shape[1], 2 if t_down else 1, 2 if down else 1)
-        return x, dims
+    def _head(self, L: Layer, x: Tensor, dims, out: Tensor) -> None:
+        """encoder.head + conv1 (mu half) into `out`, this chunk's latent-frame window of the result."""
+        y = self._conv(L.name, self._act(x, dims, "encoder.head.0", True, key=L.name), dims, key=L.name)
+        w1, b1 = self.lin["conv1"]
+        mu = self._new(y.shape[0], w1.shape[0], dtype=_F32)
+        ops.gemm(y, w1, b1, mu, ops.YB_EPI_F32)
+        if self._one_pass:
+            ops.nhwc_to_nchw_f32(mu, out.view(self.z_dim, -1))
+        else:
+            ops.nhwc_to_nchw_f32_win(mu, out)
 
     def _frames(self, video: Tensor) -> Tensor:
         if video.dim() != 4 or video.shape[0] != 3:
             raise YumeB200Error("expected a video [3, T, H, W]")
         keep = 1 + 4 * ((video.shape[1] - 1) // 4)                 # `iter_ = 1 + (t - 1) // 4` chunks of 1, 4, 4, ... (:802-803)
         return video[:, :keep].to(self.device, _F32).contiguous()
-
-    def _head(self, x: Tensor, dims, out: Tensor) -> None:
-        """encoder.head + conv1 (mu half) into `out`, this chunk's latent-frame window of the result."""
-        k = "encoder.head.2"
-        y = self._conv(k, self._act(x, dims, "encoder.head.0", True, key=k), dims, key=k)
-        w1, b1 = self.lin["conv1"]
-        mu = self._new(y.shape[0], w1.shape[0], dtype=_F32)
-        ops.gemm(y, w1, b1, mu, ops.YB_EPI_F32)
-        if self._chunk == 0 and not self._more:
-            ops.nhwc_to_nchw_f32(mu, out.view(self.z_dim, -1))
-        else:
-            ops.nhwc_to_nchw_f32_win(mu, out)
-
-    def _middle(self, x: Tensor, dims) -> Tensor:
-        x = self._res_block("encoder.middle.0", x, dims)
-        x = self._attention("encoder.middle.1", x, dims)
-        return self._res_block("encoder.middle.2", x, dims)
-
-    # ---- chunk streaming -----------------------------------------------------------------------------------
-    SCALE = 16                                                     # spatial downsampling of the latent
-
-    def _check_hw(self, H: int, W: int) -> None:
-        if H % 16 or W % 16:
-            raise YumeB200Error("Wan2.2 VAE encode needs H, W divisible by 16 (patchify 2 x three stride-2 levels)")
-
-    def _input(self, v: Tensor):
-        """encoder.conv1's input buffer (carried frames in front) with this chunk's patchified frames behind them."""
-        _, T, H, W = v.shape
-        dims = (T, H // 2, W // 2)
-        x0 = self._hist_buf("encoder.conv1", *dims, 64)
-        dst = x0[x0.shape[0] - T:].view(-1, 64)
-        if self._chunk == 0 and not self._more:
-            ops.vae_patchify2_bf16(v, dst)
-        else:
-            ops.vae_patchify2_bf16_win(v, dst)
-        return x0, dims
-
-    def _encode_chunk(self, v: Tensor, out: Tensor) -> None:
-        x0, dims = self._input(v)
-        x = self._conv("encoder.conv1", x0, dims, key="encoder.conv1")
-        for i in range(self.n_down):
-            x, dims = self._down_block(i, x, dims)
-        self._head(self._middle(x, dims), dims, out)
 
     @torch.no_grad()
     def encode(self, video: Tensor) -> Tensor:
@@ -229,114 +194,71 @@ class Wan22VaeEncoder(Wan22VaeDecoder):
         frames, every later one 4n (the reference's frame 0, then 4 frames per call)."""
         video = self._frames(video)
         _, T, H, W = video.shape
-        self._check_hw(H, W)
-        Tl = 1 + (T - 1) // 4
-        if sum(lengths) != Tl or min(lengths) < 1:
-            raise YumeB200Error(f"chunk lengths {list(lengths)} do not partition {Tl} latent frames")
-        out = self._new(self.z_dim, Tl, H // self.SCALE, W // self.SCALE, dtype=_F32)
-        t0, f0 = 0, 0
-        self._carry = {}
-        try:
-            for i, n in enumerate(lengths):
-                self._chunk, self._more = i, i < len(lengths) - 1
-                nv = 1 + 4 * (n - 1) if i == 0 else 4 * n
-                self._encode_chunk(video[:, f0:f0 + nv], out[:, t0:t0 + n])
-                t0, f0 = t0 + n, f0 + nv
-        finally:
-            self._chunk, self._more, self._carry = 0, False, None
-        return out
+        if H % self.SCALE or W % self.SCALE:
+            raise YumeB200Error(f"Wan VAE encode needs H, W divisible by {self.SCALE}")
+        return self._chunks(video, lengths, (self.z_dim, 1 + (T - 1) // 4, H // self.SCALE, W // self.SCALE), 4, 1)
 
     def _fixed_bytes(self, T: int, H: int, W: int) -> int:
         """mu, and the device copy of the video `encode` makes when it is handed one on another device or not contiguous."""
         return 4 * (self.z_dim * (1 + (T - 1) // 4) * (H // self.SCALE) * (W // self.SCALE) + 3 * T * H * W)
 
-    def _level_plan(self, H: int, W: int) -> List[tuple]:
-        """The encoder's layer plan at video size H x W, frames per latent frame of a chunk first (see Wan22VaeDecoder)."""
-        d, s, h, w = self.dims, 4, H // 2, W // 2
-        plan: List[tuple] = [("in", s, h, w, 64, d[0])]
-        for i in range(self.n_down):
-            for j in range(self.nrb):
-                plan.append(("res", s, h, w, d[i] if j == 0 else d[i + 1], d[i + 1]))
-            if i != self.n_down - 1:
-                t = i < len(self.t_down) and self.t_down[i]
-                plan.append(("down", s, h, w, d[i + 1], t, d[i]))
-                s, h, w = (s // 2 if t else s), h // 2, w // 2
-        return plan + self._tail_plan(s, h, w, d[-1])
-
-    def _tail_plan(self, s: int, h: int, w: int, c: int) -> List[tuple]:
-        return [("res", s, h, w, c, c), ("attn", s, h, w, c, 0), ("res", s, h, w, c, c),
-                ("head", s, h, w, c, _rup(2 * self.z_dim, 32) + 2 * _rup(self.z_dim, 32))]
-
     def plan_chunks(self, T: int, H: int, W: int) -> List[int]:
-        """Latent frames per chunk of an encode of T video frames at H x W (see Wan22VaeDecoder._plan)."""
+        """Latent frames per chunk of an encode of T video frames at H x W (see _plan)."""
         return self._plan(1 + (T - 1) // 4, lambda n: self.chunk_bytes(n, T, H, W))
 
-    def decode(self, z):                                           # the inherited decoder entry point has no weights here
-        raise YumeB200Error("this engine holds the encoder side; use Wan22VaeDecoder for decode")
+
+class Wan22VaeEncoder(WanVaeEncoder):
+    """`Wan2_2_VAE.encode` for one video: f32 [3, T, H, W] -> mu f32 [z_dim, 1 + (T-1)//4, H/16, W/16]."""
+    SCALE = 16                                                     # patchify 2 x three stride-2 levels
+
+    def __init__(self, sd: Dict[str, Tensor], dim: int = 160, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
+                 num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
+        dims = [dim * u for u in [1] + list(dim_mult)]                               # vae2_2.py:527
+        layers = [Layer("in", "encoder.conv1", 64, dims[0], 4, 2)]
+        for i in range(len(dim_mult)):                             # Down_ResidualBlock (:420-459)
+            p, ci, co = f"encoder.downsamples.{i}.downsamples", dims[i], dims[i + 1]
+            down = i != len(dim_mult) - 1
+            ft = 2 if i < len(temperal_downsample) and temperal_downsample[i] else 1
+            layers.append(Layer("hold", ci=ci))
+            layers += [Layer("res", f"{p}.{j}", ci if j == 0 else co, co) for j in range(num_res_blocks)]
+            if down:
+                layers.append(Layer("down", f"{p}.{num_res_blocks}", co, co, ft, 2))
+            layers.append(Layer("avgdown", ci=ci, co=co, ft=ft, fs=2 if down else 1))
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device)
+
+    def _read(self, v: Tensor, dst: Tensor) -> None:
+        if self._one_pass:
+            ops.vae_patchify2_bf16(v, dst)
+        else:
+            ops.vae_patchify2_bf16_win(v, dst)
 
 
-class Wan21VaeEncoder(Wan22VaeEncoder):
+class Wan21VaeEncoder(WanVaeEncoder):
     """`WanVAE.encode` (wan/modules/vae.py:515-542, 645-653): f32 [3, T, H, W] -> mu f32 [16, 1 + (T-1)//4, H/8, W/8]. Flat
     `encoder.downsamples` Sequential (:293-306), no AvgDown3D shortcut, RGB straight into `encoder.conv1`."""
+    SCALE = 8
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
                  mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
-        self.device = torch.device(device)
-        self.z_dim = z_dim
-        self.enc_dims = dims = [dim * u for u in [1] + list(dim_mult)]
-        self.plan, n = [], 0
+        dims = [dim * u for u in [1] + list(dim_mult)]
+        layers, n = [Layer("in", "encoder.conv1", 64, dims[0], 4, 1)], 0
         for i in range(len(dim_mult)):
+            ci, co = dims[i], dims[i + 1]
             for _ in range(num_res_blocks):
-                self.plan.append((n, "res"))
-                n += 1
+                layers.append(Layer("res", f"encoder.downsamples.{n}", ci, co))
+                n, ci = n + 1, co
             if i != len(dim_mult) - 1:
-                self.plan.append((n, "downsample3d" if temperal_downsample[i] else "downsample2d"))
+                layers.append(Layer("down", f"encoder.downsamples.{n}", co, co, 2 if temperal_downsample[i] else 1, 2))
                 n += 1
-        mean = torch.zeros(z_dim) if mean is None else mean
-        std = torch.ones(z_dim) if std is None else std
-        self._repack_encoder(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32), dims[-1])
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device)
 
-    SCALE = 8
-
-    def _check_hw(self, H: int, W: int) -> None:
-        if H % 8 or W % 8:
-            raise YumeB200Error("Wan2.1 VAE encode needs H, W divisible by 8")
-
-    def _input(self, v: Tensor):
-        _, T, H, W = v.shape
-        x0 = self._hist_buf("encoder.conv1", T, H, W, 64)
-        dst = x0[x0.shape[0] - T:].view(-1, 64)
-        if self._chunk == 0 and not self._more:
+    def _read(self, v: Tensor, dst: Tensor) -> None:
+        if self._one_pass:
             ops.nchw_to_nhwc_bf16(v.view(3, -1), dst)
         else:
             ops.nchw_to_nhwc_bf16_win(v, dst)
-        return x0, (T, H, W)
-
-    def _encode_chunk(self, v: Tensor, out: Tensor) -> None:
-        x0, dims = self._input(v)
-        x = self._conv("encoder.conv1", x0, dims, key="encoder.conv1")
-        for n, kind in self.plan:
-            p = f"encoder.downsamples.{n}"
-            if kind == "res":
-                x = self._res_block(p, x, dims)
-            else:
-                x, dims = self._resample_down(p, x, dims, kind == "downsample3d")
-        self._head(self._middle(x, dims), dims, out)
-
-    def _level_plan(self, H: int, W: int) -> List[tuple]:
-        d, s, h, w = self.enc_dims, 4, H, W
-        plan: List[tuple] = [("in", s, h, w, 64, d[0])]
-        level, c = 0, d[0]
-        for _, kind in self.plan:
-            if kind == "res":
-                plan.append(("res", s, h, w, c, d[level + 1]))
-                c = d[level + 1]
-            else:
-                t = kind == "downsample3d"
-                plan.append(("down", s, h, w, c, t, 0))
-                s, h, w, level = (s // 2 if t else s), h // 2, w // 2, level + 1
-        return plan + self._tail_plan(s, h, w, c)
 
 
 def install_wan22_vae_encoder(vae, device="cuda"):

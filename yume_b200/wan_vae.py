@@ -1,0 +1,337 @@
+"""What the four Wan VAE engines share — `Wan22VaeDecoder` (vae22.py), `Wan21VaeDecoder` (vae21.py) and the two encoders
+(vae_enc.py): weight re-packing, the building blocks (causal conv, RMS_norm + SiLU, ResidualBlock, the mid attention), the conv
+history carried from chunk to chunk, and the chunk driver and planner. Each engine describes its network once, as a layer list
+built from its config: `_run_chunk` walks it to run a chunk and `chunk_bytes` walks it to bound one.
+"""
+from __future__ import annotations
+
+from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
+
+import torch
+
+from ._lib import YumeB200Error
+
+Tensor = torch.Tensor
+_BF16, _F32 = torch.bfloat16, torch.float32
+
+
+def _rup(v: int, m: int) -> int:
+    return (v + m - 1) // m * m
+
+
+class Layer(NamedTuple):
+    """One step of an engine's layer list. `hold` keeps the level's input for the DupUp3D / AvgDown3D shortcut that ends the
+    level (`dupup`, `avgdown`)."""
+    kind: str               # in | res | attn | hold | up | down | dupup | avgdown | head
+    name: str = ""          # module prefix in the state dict
+    ci: int = 0             # input channels (hold: those of the held input)
+    co: int = 0             # output channels (head: the output columns the planner counts at 4 bytes)
+    ft: int = 1             # in: frames per latent frame; up / down / shortcut: time factor
+    fs: int = 1             # in: patch size; up / down / shortcut: space factor
+
+
+class WanVaeEngine:
+    """Base of the four engines. An engine builds its layer list from its config and hands it to this constructor; its side
+    (decode or encode) supplies `_repack`, the `in`, `up` / `down` and `head` steps (`_input`, `_resample`, `_head`) and `ops`,
+    the op library of its own module (which tests replace, module by module, with a CPU stand-in)."""
+    # chunk-streaming state of the running call: chunk index, whether another chunk follows, carried conv input frames
+    _chunk, _more, _carry = 0, False, None
+    HIST = 2                     # carried frames of a 3-tap causal conv (the reference's CACHE_T)
+    MEM_MARGIN = 2 << 30         # bytes of free device memory the chunk planner leaves unused
+
+    def __init__(self, sd: Dict[str, Tensor], z_dim: int, layers: List[Layer], mean: Optional[Tensor], std: Optional[Tensor],
+                 device):
+        self.device = torch.device(device)
+        self.z_dim, self.layers = z_dim, layers
+        mean = torch.zeros(z_dim) if mean is None else mean
+        std = torch.ones(z_dim) if std is None else std
+        self._repack(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32))
+
+    # ---- weights -------------------------------------------------------------------------------------------
+    def _pack_side(self, sd: Dict[str, Tensor], prefixes: Tuple[str, ...], latent_conv: str,
+                   split_time_conv: bool) -> Dict[str, Tensor]:
+        """Re-pack one side of a `WanVAE_` state dict (decode: `decoder.*` + `conv2`; encode: `encoder.*` + `conv1`): 3-D / 2-D
+        convs as [cop, taps*cp] bf16 GEMM weights, 1x1x1 shortcuts as plain matrices, gammas flat, the mid attention with the
+        softmax scale folded into q and the v bias folded through `proj`. Returns the fp32 device copy of that side."""
+        dev = self.device
+        sd = {k: v.detach().to(dev, _F32) for k, v in sd.items() if k.startswith(prefixes)}
+        self.conv: Dict[str, Tuple[Tensor, Tensor, tuple]] = {}    # name -> (w bf16 [cop, taps*cp], bias f32 [cop], taps)
+        self.lin: Dict[str, Tuple[Tensor, Tensor]] = {}            # 1x1x1 convs as plain GEMM weights
+        self.gamma: Dict[str, Tensor] = {}
+
+        def pack_conv(name: str, w: Tensor, b: Tensor) -> None:
+            w = w.detach().float()
+            if w.dim() == 4:                                        # Conv2d [co, ci, kh, kw] -> taps (1, kh, kw)
+                w = w.unsqueeze(2)
+            co, ci, kt, kh, kw = w.shape
+            cop, cp = _rup(co, 32), _rup(ci, 64)
+            wt = torch.zeros(cop, kt * kh * kw, cp, dtype=_F32, device=dev)
+            wt[:co, :, :ci] = w.permute(0, 2, 3, 4, 1).reshape(co, kt * kh * kw, ci)
+            bp = torch.zeros(cop, dtype=_F32, device=dev)
+            bp[:co] = b.detach().float()
+            self.conv[name] = (wt.reshape(cop, -1).to(dev, _BF16).contiguous(), bp.to(dev), (kt, kh, kw))
+
+        latent_w = latent_conv + ".weight"
+        for k, v in sd.items():
+            if k.endswith(".gamma"):
+                self.gamma[k[:-6]] = v.detach().to(dev, _F32).reshape(-1).contiguous()
+            elif k.endswith(".weight") and v.dim() == 5 and tuple(v.shape[2:]) == (1, 1, 1) and k != latent_w:
+                name = k[:-7]                                       # ResidualBlock.shortcut: plain GEMM
+                co, ci = v.shape[:2]
+                w = torch.zeros(_rup(co, 32), _rup(ci, 8), dtype=_F32, device=dev)
+                w[:co, :ci] = v.detach().float().reshape(co, ci)
+                b = torch.zeros(_rup(co, 32), dtype=_F32, device=dev)
+                b[:co] = sd[name + ".bias"].detach().float()
+                self.lin[name] = (w.to(dev, _BF16).contiguous(), b.to(dev))
+            elif k.endswith(".time_conv.weight") and split_time_conv:
+                name = k[:-7]
+                C2 = v.shape[0]
+                for g in (0, 1):                                    # the two channel groups become two output frames
+                    pack_conv(f"{name}.{g}", v[g * C2 // 2:(g + 1) * C2 // 2], sd[name + ".bias"][g * C2 // 2:(g + 1) * C2 // 2])
+            elif k.endswith(".weight") and v.dim() in (4, 5) and "to_qkv" not in k and ".proj." not in k and k != latent_w:
+                pack_conv(k[:-7], v, sd[k[:-7] + ".bias"])
+        # attention: scale folded into q; v bias folded through proj (softmax rows sum to 1)
+        attn = next(L for L in self.layers if L.kind == "attn")
+        C, p = attn.ci, attn.name
+        Wqkv = sd[p + ".to_qkv.weight"].detach().float().reshape(3 * C, C)
+        bqkv = sd[p + ".to_qkv.bias"].detach().float()
+        Wo = sd[p + ".proj.weight"].detach().float().reshape(C, C)
+        scale = C ** -0.5
+        self.att = dict(wq=(Wqkv[:C] * scale).to(dev, _BF16).contiguous(), bq=(bqkv[:C] * scale).to(dev),
+                        wk=Wqkv[C:2 * C].to(dev, _BF16).contiguous(), bk=bqkv[C:2 * C].to(dev).contiguous(),
+                        wv=Wqkv[2 * C:].to(dev, _BF16).contiguous(),
+                        wo=Wo.to(dev, _BF16).contiguous(),
+                        bo=(sd[p + ".proj.bias"].detach().float() + Wo @ bqkv[2 * C:]).to(dev).contiguous())
+        return sd
+
+    # ---- building blocks -----------------------------------------------------------------------------------
+    def _new(self, *shape, dtype=_BF16) -> Tensor:
+        return torch.empty(*shape, device=self.device, dtype=dtype)
+
+    @property
+    def _one_pass(self) -> bool:
+        """The running chunk is the whole sequence: it issues the one-pass launches."""
+        return self._chunk == 0 and not self._more
+
+    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0) -> Tensor:
+        """Input buffer [h + T, H, W, Cp] of a conv whose input stream is `key`: after the first chunk its first h frames (n, or
+        HIST when n is 0) are the frames carried from the previous chunk and the producer writes the T new frames behind them."""
+        h = (n or self.HIST) if (key is not None and self._chunk > 0) else 0
+        buf = torch.zeros(h + T, H, W, Cp, device=self.device, dtype=_BF16) if zero else self._new(h + T, H, W, Cp)
+        if h:
+            buf[:h].copy_(self._carry[key])
+        return buf
+
+    def _keep(self, key: str, frames: Tensor, n: int = 0) -> None:
+        """Carry the last n (0: HIST) frames of the input stream `key` into the next chunk (zero frames in front where the stream
+        is shorter: the causal zero padding)."""
+        if not self._more:
+            return
+        n = n or self.HIST
+        if frames.shape[0] >= n:
+            self._carry[key] = frames[frames.shape[0] - n:].clone()
+        else:
+            c = torch.zeros(n, *frames.shape[1:], device=self.device, dtype=_BF16)
+            c[n - frames.shape[0]:].copy_(frames)
+            self._carry[key] = c
+
+    def _conv(self, name: str, a: Tensor, dims, epilogue=None, res: Optional[Tensor] = None, out: Optional[Tensor] = None,
+              out_t_mul: int = 1, out_t_add: int = 0, stride_t: int = 1, stride_hw: int = 1, key: Optional[str] = None) -> Tensor:
+        """a bf16 [h + T, H, W, Cp] (unpadded, dense; h carried frames in front, see _hist_buf) -> [To*Ho*Wo (or interleaved
+        frames), cop]. `key`: the input stream whose last frames the next chunk needs."""
+        ops = self.ops
+        w, b, taps = self.conv[name]
+        T, H, W = dims
+        h = a.shape[0] - T
+        if key is not None:                                      # a stride-2 time_conv carries one frame (vae2_2.py:158-170)
+            self._keep(key, a, 1 if stride_t > 1 else self.HIST)
+        if epilogue is None:
+            epilogue = ops.YB_EPI_RES_BF16 if res is not None else ops.YB_EPI_BF16
+        if out is None:
+            To, Ho, Wo = ops.conv_out_dims(T, H, W, taps, stride_t, stride_hw)
+            out = self._new(To * Ho * Wo, w.shape[0], dtype=_F32 if epilogue == ops.YB_EPI_F32 else _BF16)
+        if h:
+            ops.conv3d_causal_hist(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, out_t_mul=out_t_mul,
+                                   out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
+        else:
+            ops.conv3d_causal(a, w, b, out, T, H, W, epilogue, res, taps=taps, oob_zero_pad=True, out_t_mul=out_t_mul,
+                              out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
+        return out
+
+    def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1, key: Optional[str] = None,
+             n: int = 0) -> Tensor:
+        ops = self.ops
+        T, H, W = dims
+        out = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n)
+        ops.vae_rms_act(x, dims, out[out.shape[0] - T:], self.gamma[gamma] if gamma else None, up, silu)
+        return out
+
+    def _res_block(self, p: str, x: Tensor, dims) -> Tensor:
+        """ResidualBlock (vae2_2.py:195-239)."""
+        ops = self.ops
+        c1, c2 = p + ".residual.2", p + ".residual.6"
+        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1), dims, key=c1)
+        res = x
+        if (p + ".shortcut") in self.lin:
+            w, b = self.lin[p + ".shortcut"]
+            res = self._new(x.shape[0], w.shape[0])
+            ops.gemm(x, w, b, res, ops.YB_EPI_BF16)
+        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2), dims, res=res, key=c2)
+
+    def _attention(self, p: str, x: Tensor, dims) -> Tensor:
+        """AttentionBlock (vae2_2.py:242-283): per-frame single-head attention over H*W tokens, d = C."""
+        ops = self.ops
+        T, H, W = dims
+        N, C = x.shape
+        HW = H * W
+        Lf = _rup(HW, 32)                                        # per-frame key count padded for the GEMM tile
+        a = self.att
+        S, P, o = self._new(HW, Lf, dtype=_F32), self._new(HW, Lf), self._new(N, C)
+        if HW % 8:
+            # frames whose H*W rows are not 16-byte multiples in the transposed V (tiny latents only): every frame gets its own
+            # zero-padded Lf-row slot, so per-frame slices of q, k and v^T start on aligned addresses
+            tmp = self._new(T, H, W, C)
+            ops.vae_rms_act(x, dims, tmp, self.gamma[p + ".norm"], 1, False)
+            hn = torch.zeros(T * Lf + 32, C, device=self.device, dtype=_BF16)
+            hn[:T * Lf].view(T, Lf, C)[:, :HW].copy_(tmp.view(T, HW, C))
+            q, k, vT = self._new(T * Lf, C), self._new(T * Lf, C), self._new(C, T * Lf + 32)
+            ops.gemm(hn[:T * Lf], a["wq"], a["bq"], q, ops.YB_EPI_BF16)
+            ops.gemm(hn[:T * Lf], a["wk"], a["bk"], k, ops.YB_EPI_BF16)
+            ops.gemm(a["wv"], hn, None, vT, ops.YB_EPI_BF16)
+            for f in range(T):
+                ops.gemm(q[f * Lf:f * Lf + HW], k[f * Lf:(f + 1) * Lf], None, S, ops.YB_EPI_F32)
+                ops.masked_softmax(S, P, HW, HW)
+                ops.gemm(P, vT[:, f * Lf:(f + 1) * Lf], None, o[f * HW:(f + 1) * HW], ops.YB_EPI_BF16)
+        else:
+            Next = _rup(N, 32) + 32
+            hn = torch.zeros(Next, C, device=self.device, dtype=_BF16)
+            ops.vae_rms_act(x, dims, hn[:N].view(T, H, W, C), self.gamma[p + ".norm"], 1, False)
+            q, k = self._new(N, C), torch.zeros(Next, C, device=self.device, dtype=_BF16)
+            ops.gemm(hn[:N], a["wq"], a["bq"], q, ops.YB_EPI_BF16)
+            ops.gemm(hn[:N], a["wk"], a["bk"], k[:N], ops.YB_EPI_BF16)
+            vT = self._new(C, Next)
+            ops.gemm(a["wv"], hn, None, vT, ops.YB_EPI_BF16)
+            for f in range(T):
+                ops.gemm(q[f * HW:(f + 1) * HW], k[f * HW:f * HW + Lf], None, S, ops.YB_EPI_F32)
+                ops.masked_softmax(S, P, HW, HW)                 # keys >= HW (padding / next frame) get probability 0
+                ops.gemm(P, vT[:, f * HW:f * HW + Lf], None, o[f * HW:(f + 1) * HW], ops.YB_EPI_BF16)
+        out = self._new(N, C)
+        ops.gemm(o, a["wo"], a["bo"], out, ops.YB_EPI_RES_BF16, res=x)
+        return out
+
+    # ---- chunk streaming -----------------------------------------------------------------------------------
+    def _run_chunk(self, src: Tensor, out: Tensor) -> None:
+        """Run one chunk of the input, `src`, through the layer list into `out`, its frame window of the result."""
+        ops = self.ops
+        for L in self.layers:
+            if L.kind == "in":
+                x, dims = self._input(L, src)
+            elif L.kind == "res":
+                x = self._res_block(L.name, x, dims)
+            elif L.kind == "attn":
+                x = self._attention(L.name, x, dims)
+            elif L.kind == "hold":
+                held, held_dims = x, dims
+            elif L.kind in ("up", "down"):
+                x, dims = self._resample(L, x, dims)
+            elif L.kind == "dupup":                              # DupUp3D drops frames in the first chunk only (:495-503)
+                dupup = ops.vae_dupup_add if self._chunk == 0 else ops.vae_dupup_add_cont
+                dupup(x, held, held_dims, L.ci, L.co, L.ft, L.fs)
+                held = None
+            elif L.kind == "avgdown":
+                ops.vae_avgdown_add(x, held, held_dims, held.shape[1], x.shape[1], L.ft, L.fs)
+                held = None
+            else:
+                self._head(L, x, dims, out)
+
+    def _chunks(self, src: Tensor, lengths: Sequence[int], out_shape, k_in: int, k_out: int) -> Tensor:
+        """Run `src` in chunks of `lengths` latent frames into one preallocated f32 result of `out_shape`. A chunk of n latent
+        frames reads n * k_in frames of `src` and writes n * k_out frames of the result, the first chunk k - 1 fewer of each
+        (frame 0 stands alone)."""
+        units = 1 + (src.shape[1] - 1) // k_in
+        if sum(lengths) != units or min(lengths) < 1:
+            raise YumeB200Error(f"chunk lengths {list(lengths)} do not partition {units} latent frames")
+        out = self._new(*out_shape, dtype=_F32)
+        t_in, t_out = 0, 0
+        self._carry = {}
+        try:
+            for i, n in enumerate(lengths):
+                self._chunk, self._more = i, i < len(lengths) - 1
+                n_in, n_out = (n * k_in, n * k_out) if i else (1 + (n - 1) * k_in, 1 + (n - 1) * k_out)
+                self._run_chunk(src[:, t_in:t_in + n_in], out[:, t_out:t_out + n_out])
+                t_in, t_out = t_in + n_in, t_out + n_out
+        finally:
+            self._chunk, self._more, self._carry = 0, False, None
+        return out
+
+    # ---- chunk planner -------------------------------------------------------------------------------------
+    def chunk_bytes(self, n: int, T: int, H: int, W: int) -> int:
+        """Upper bound of the device bytes a decode (encode) of T latent (video) frames at H x W allocates on top of the weights
+        and its input when its chunks hold n latent frames: the whole result, every carried history, and the largest set of
+        activations one step of the layer list keeps live (every buffer of that step counted as live at once; a chunk after
+        the first is counted, it has the most frames at each level). The shortcut steps add no bytes of their own: `up` and
+        `down` count the held level input."""
+        bf, f4 = 2, 4
+        hist = self.HIST
+        carries, peak, held = 0, 0, 0
+        for L in self.layers:
+            if L.kind == "in":                                   # frames per latent frame, input size
+                s, h, w = L.ft, H // L.fs, W // L.fs
+            F, vox = n * s, h * w
+            c, co = L.ci, L.co
+            cp = _rup(c, 64)
+            live = 0
+            if L.kind == "in":                                   # input gather, conv1's input buffer (history in front), its out
+                carries += hist * vox * c * bf
+                live = (F * vox * c + (F + hist) * vox * c + F * vox * co) * bf
+            elif L.kind == "hold":
+                held = c
+            elif L.kind == "down":                               # x, held block input, act, resample.1 out (+1 carried frame),
+                vq = (h // 2) * (w // 2)                         # its act, time_conv out
+                live = (F * vox * (c + held + cp) + (F + 1) * vq * (c + cp) + F * vq * c) * bf
+                if L.ft == 2:
+                    carries += vq * cp * bf
+                s, h, w = s // L.ft, h // L.fs, w // L.fs
+            elif L.kind == "res":                                # x, the block input a shortcut add holds, y, res, out, two acts
+                carries += hist * vox * (cp + _rup(co, 64)) * bf
+                live = F * vox * (2 * c + 3 * co) * bf + (F + hist) * vox * (cp + _rup(co, 64)) * bf
+            elif L.kind == "attn":
+                Lf, Next = _rup(vox, 32), _rup(F * vox, 32) + 32
+                live = (F * vox * c * 5 + Next * c * 3 + F * Lf * c * 3) * bf + vox * Lf * (f4 + bf)
+            elif L.kind == "up":
+                t_up = L.ft == 2
+                F2 = 2 * F if t_up else F
+                live = (F * vox * (c + held) + F2 * vox * c) * bf + (F + hist) * vox * cp * bf * (1 if t_up else 0)
+                live += F2 * 4 * vox * (cp + _rup(co, 32)) * bf
+                if t_up:
+                    carries += hist * vox * cp * bf
+                s, h, w = s * L.ft, h * L.fs, w * L.fs
+            elif L.kind in ("dupup", "avgdown"):
+                held = 0
+            elif L.kind == "head":                               # act, f32 conv output
+                live = (F * vox * c + (F + hist) * vox * cp) * bf + F * vox * co * f4
+                carries += hist * vox * cp * bf
+            peak = max(peak, live)
+        return self._fixed_bytes(T, H, W) + carries + peak
+
+    def _plan(self, units: int, nbytes) -> List[int]:
+        """Latent frames per chunk: all `units` when they fit (and always off CUDA), else the longest chunks whose `nbytes`
+        fit the device's free memory (free + torch's cached, unallocated blocks) minus MEM_MARGIN. The free memory is read
+        when the call starts, so other work on the same GPU can make a sequence that would fit alone run in chunks (with the
+        same result)."""
+        if self.device.type != "cuda":
+            return [units]
+        free, _ = torch.cuda.mem_get_info(self.device)
+        free += torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+        return chunk_lengths(units, nbytes, free - self.MEM_MARGIN)
+
+
+def chunk_lengths(T: int, nbytes, budget: int) -> List[int]:
+    """Partition T latent frames into chunks of the longest length n whose `nbytes(n)` (non-decreasing in n) fits `budget`, the
+    last chunk taking the remainder: [T] when the whole sequence fits, chunks of 1 frame when nothing longer does."""
+    if nbytes(T) <= budget:
+        return [T]
+    n = 1
+    while n + 1 < T and nbytes(n + 1) <= budget:
+        n += 1
+    return [n] * (T // n) + ([T % n] if T % n else [])
