@@ -123,6 +123,28 @@ STREAM_SIGNATURES = {
     "yb_nchw_to_nhwc_bf16_win": (_i, [_vp, _ll, _vp, _ll, _i, _i, _vp]),
 }
 
+# every symbol include/yume_b200_fp8.h declares (the opt-in FP8 block GEMMs and their activation quantisers)
+YB_EPI_GELU_FP8 = 8
+
+
+class GemmFp8Args(C.Structure):
+    """Mirror of `struct yb_gemm_fp8_args` (include/yume_b200_fp8.h)."""
+
+    _fields_ = [
+        ("struct_bytes", C.c_uint), ("M", C.c_int), ("N", C.c_int), ("K", C.c_int),
+        ("A", C.c_void_p), ("a_scale", C.c_void_p), ("B", C.c_void_p), ("b_scale", C.c_void_p), ("bias", C.c_void_p),
+        ("out", C.c_void_p), ("out_scale", C.c_void_p), ("gate", C.c_void_p), ("tok_idx", C.c_void_p),
+        ("lda", C.c_longlong), ("lds", C.c_longlong), ("ldb", C.c_longlong), ("ldo", C.c_longlong), ("ldos", C.c_longlong),
+        ("gate_ld", C.c_longlong), ("epilogue", C.c_int), ("block_n", C.c_int),
+    ]
+
+
+FP8_SIGNATURES = {
+    "yb_gemm_fp8": (_i, [C.POINTER(GemmFp8Args), _vp]),
+    "yb_ln_modulate_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _ll, _vp, _vp, _vp, _i, _i, _f, _vp]),
+    "yb_quant_rows_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
+}
+
 _lib = None
 
 
@@ -143,7 +165,8 @@ def load():
     if lib.yb_abi_version() != ABI_VERSION:
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
-    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES}.items():
+    for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
+                              **FP8_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

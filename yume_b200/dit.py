@@ -105,6 +105,21 @@ def framepack_plan(hist: int, branch_hist: int) -> List[_Segment]:
     return segs
 
 
+FP8_MAX = 448.0                                  # largest finite e4m3 value
+FP8_WEIGHTS = ("w_qkv", "w_o", "cw_q", "cw_o", "w1", "w2")   # the block linears that precision="fp8" converts
+FP8_LN_WIDTHS = (256, 1024, 3072, 5120)          # model widths yb_ln_modulate_fp8 has an instance for
+
+
+def quantize_weight_fp8(w: Tensor) -> Tuple[Tensor, Tensor]:
+    """Per-output-channel e4m3 weight (include/yume_b200_fp8.h): s_w[n] = amax_n / 448, Wq = e4m3(clamp(W * 448 / amax_n,
+    +-448)); an all-zero row gets s_w = 0 and Wq = 0. w [N, K] any float dtype -> (Wq float8_e4m3fn [N, K], s_w f32 [N])."""
+    w = w.float()
+    amax = w.abs().amax(dim=1)
+    mult = torch.where(amax > 0, FP8_MAX / amax, torch.zeros_like(amax))
+    wq = (w * mult[:, None]).clamp(-FP8_MAX, FP8_MAX).to(torch.float8_e4m3fn).contiguous()
+    return wq, (amax / torch.full_like(amax, FP8_MAX)).contiguous()   # tensor / tensor: IEEE division, as on every device
+
+
 def sp_qkv_row_order(dim: int, heads: int, world: int) -> Tensor:
     """Row permutation of the fused [3C, C] q|k|v weight for Ulysses: [peer][part q,k,v][that peer's heads]."""
     wh = (heads // world) * (dim // heads)
@@ -125,9 +140,16 @@ class WanDiT:
 
     def __init__(self, state_dict: Dict[str, Tensor], variant: str, dim: int, ffn_dim: int, num_heads: int,
                  num_layers: int, in_dim: int, out_dim: int, text_len: int = 512, freq_dim: int = 256,
-                 patch_size: Sequence[int] = (1, 2, 2), eps: float = 1e-6, device: str | torch.device = "cuda"):
+                 patch_size: Sequence[int] = (1, 2, 2), eps: float = 1e-6, device: str | torch.device = "cuda",
+                 precision: str = "bf16"):
         if variant not in ("5b", "14b"):
             raise YumeB200Error("variant must be '5b' or '14b'")
+        if precision not in ("bf16", "fp8"):
+            raise YumeB200Error("precision must be 'bf16' or 'fp8'")
+        if precision == "fp8" and (dim % 128 or ffn_dim % 128):
+            raise YumeB200Error(f"precision='fp8' needs dim and ffn_dim divisible by 128 (1x128 scale groups), got {dim}, {ffn_dim}")
+        if precision == "fp8" and dim not in FP8_LN_WIDTHS:
+            raise YumeB200Error(f"precision='fp8' runs the fp8 LayerNorm at dim {FP8_LN_WIDTHS} only, got {dim}")
         if tuple(patch_size) != (1, 2, 2):
             raise YumeB200Error("only patch_size (1, 2, 2) is supported (both Yume models use it)")
         if dim % num_heads or dim // num_heads != 128:
@@ -136,6 +158,9 @@ class WanDiT:
         self.in_dim, self.out_dim, self.text_len, self.freq_dim, self.eps = in_dim, out_dim, text_len, freq_dim, eps
         self.device = torch.device(device)
         self.head_dim = 128
+        # "fp8": the six block linears (q|k|v, o, cross q, cross o, ffn.0, ffn.2) run as e4m3 GEMMs with per-channel weight
+        # scales and 1x128 activation scales (include/yume_b200_fp8.h); everything else stays as in "bf16"
+        self.precision = precision
         self._ws: Dict[Tuple, Tensor] = {}
         self._rope_cache: Dict[Tuple, Tensor] = {}
         self.timer = KernelTimer()          # bench.py switches it on to time individual kernels inside a live step
@@ -170,6 +195,11 @@ class WanDiT:
         def cat32(names):
             return torch.cat([sd[n].detach().to(device=dev, dtype=_F32) for n in names], dim=0).contiguous()
 
+        def lin(names):   # one of the converted block linears: bf16, or (e4m3, s_w) quantised from the checkpoint's own values
+            if self.precision == "bf16":
+                return cat16(names)
+            return quantize_weight_fp8(cat32(names))
+
         self.embed: Dict[str, Tuple[Tensor, Tensor]] = {}
         for name in ("patch_embedding", "patch_embedding_2x", "patch_embedding_4x", "patch_embedding_8x",
                      "patch_embedding_16x", "patch_embedding_2x_f"):
@@ -197,17 +227,17 @@ class WanDiT:
             p = f"blocks.{i}"
             sa, ca = p + ".self_attn", p + ".cross_attn"
             blk = dict(
-                w_qkv=cat16([sa + ".q.weight", sa + ".k.weight", sa + ".v.weight"]),
+                w_qkv=lin([sa + ".q.weight", sa + ".k.weight", sa + ".v.weight"]),
                 b_qkv=cat32([sa + ".q.bias", sa + ".k.bias", sa + ".v.bias"]),
-                w_o=w16(sa + ".o.weight"), b_o=f32(sa + ".o.bias"),
+                w_o=lin([sa + ".o.weight"]), b_o=f32(sa + ".o.bias"),
                 nq=f32(sa + ".norm_q.weight"), nk=f32(sa + ".norm_k.weight"),
-                cw_q=w16(ca + ".q.weight"), cb_q=f32(ca + ".q.bias"),
+                cw_q=lin([ca + ".q.weight"]), cb_q=f32(ca + ".q.bias"),
                 cw_kv=cat16([ca + ".k.weight", ca + ".v.weight"]), cb_kv=cat32([ca + ".k.bias", ca + ".v.bias"]),
-                cw_o=w16(ca + ".o.weight"), cb_o=f32(ca + ".o.bias"),
+                cw_o=lin([ca + ".o.weight"]), cb_o=f32(ca + ".o.bias"),
                 cnq=f32(ca + ".norm_q.weight"), cnk=f32(ca + ".norm_k.weight"),
                 n3w=f32(p + ".norm3.weight"), n3b=f32(p + ".norm3.bias"),
-                w1=w16(p + ".ffn.0.weight"), b1=f32(p + ".ffn.0.bias"),
-                w2=w16(p + ".ffn.2.weight"), b2=f32(p + ".ffn.2.bias"),
+                w1=lin([p + ".ffn.0.weight"]), b1=f32(p + ".ffn.0.bias"),
+                w2=lin([p + ".ffn.2.weight"]), b2=f32(p + ".ffn.2.bias"),
             )
             if self.variant == "14b":
                 blk["cw_kv_img"] = cat16([ca + ".k_img.weight", ca + ".v_img.weight"])
@@ -235,6 +265,8 @@ class WanDiT:
         exactly the chunks the all-to-all sends."""
         if transport not in ("auto", "p2p", "p2p_gemm", "nccl"):
             raise YumeB200Error("transport must be auto, p2p, p2p_gemm or nccl")
+        if self.precision == "fp8":
+            raise YumeB200Error("sequence parallelism runs the bf16 block GEMMs only: build the engine with precision='bf16'")
         self.sp_transport, self._sp_p2p = transport, None
         import torch.distributed as dist
         P = dist.get_world_size(group)
@@ -268,7 +300,7 @@ class WanDiT:
             self.sp_world, self.sp_rank = saved
 
     @classmethod
-    def from_module(cls, model: torch.nn.Module, variant: str, device="cuda") -> "WanDiT":
+    def from_module(cls, model: torch.nn.Module, variant: str, device="cuda", precision: str = "bf16") -> "WanDiT":
         """Build from a live reference WanModel (or yume_b200.model.WanModel): reads its parameters, never
         modifies the checkpoint format (SURVEY.md §8b 'State-dict')."""
         sd = dict(model.state_dict())
@@ -279,7 +311,7 @@ class WanDiT:
                 sd[name + ".weight"], sd[name + ".bias"] = m.weight, m.bias
         return cls(sd, variant, dim=model.dim, ffn_dim=model.ffn_dim, num_heads=model.num_heads,
                    num_layers=model.num_layers, in_dim=model.in_dim, out_dim=model.out_dim, text_len=model.text_len,
-                   freq_dim=model.freq_dim, patch_size=model.patch_size, eps=model.eps, device=device)
+                   freq_dim=model.freq_dim, patch_size=model.patch_size, eps=model.eps, device=device, precision=precision)
 
     # ------------------------------------------------------------------------------------------------------
     # workspace / tables
@@ -584,6 +616,10 @@ class WanDiT:
     def _block(self, i: int, xs: Tensor, mod: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int,
                ctx: Tensor, L_true: Optional[int] = None) -> None:
         """One WanAttentionBlock in place on the fp32 residual stream xs [L, C] (a token shard under Ulysses)."""
+        if self.precision == "fp8":
+            return self._block_fp8(self.blocks[i], xs, mod[i], tok_idx, rope, rope_len,
+                                   ctx[i] if isinstance(ctx, list) else self._cross_kv(ctx)[i],
+                                   L_true if L_true is not None else xs.shape[0])
         b, C, H, D = self.blocks[i], self.dim, self.heads, self.head_dim
         L = xs.shape[0]
         m = mod[i]                                             # [U, 6, C]: shift_a, scale_a, gate_a, shift_f, scale_f, gate_f
@@ -643,6 +679,96 @@ class WanDiT:
         ops.gemm(hid, b["w2"], b["b2"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 5], tok_idx=tok_idx)
         T.end("gemm_ffn2")
 
+    # ------------------------------------------------------------------------------------------------------
+    # precision="fp8": the same block with e4m3 operands for the six converted linears (include/yume_b200_fp8.h)
+    # ------------------------------------------------------------------------------------------------------
+    def _act8(self, key: str, rows: int, cols: int) -> Tuple[Tensor, Tensor]:
+        """Workspace of one fp8 activation: e4m3 values [rows, cols] and their 1x128 scales f32 [cols / 128, ld >= rows]."""
+        return (self._buf(key + "_q", (rows, cols), torch.float8_e4m3fn),
+                self._buf(key + "_s", (cols // 128, ops.fp8_scale_ld(rows)), _F32))
+
+    def _block_fp8(self, b: dict, xs: Tensor, m: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int, ctx,
+                   k_len: int) -> None:
+        """One block (weights `b`, modulation rows m [U, 6, C], this block's cross K|V `ctx`) in place on xs [L, C]."""
+        C = self.dim
+        L = xs.shape[0]
+        h8 = self._act8("h8", L, C)
+        qkv = self._buf("qkv", (L, 3 * C), _BF16)
+        att = self._buf("att", (L, C), _BF16)
+        T = self.timer
+        T.begin("ln_modulate")
+        ops.ln_modulate_fp8(xs, *h8, m[:, 1], m[:, 0], tok_idx, eps=self.eps)
+        T.end("ln_modulate")
+        self._self_attention_fp8(b, h8, qkv, att, rope, rope_len, k_len, xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
+        self._cross_and_ffn_fp8(b, xs, qkv, att, m, tok_idx, ctx)
+
+    def _self_attention_fp8(self, b, h8, qkv, att, rope, rope_len, k_len, out, epilogue, gate=None, tok_idx=None) -> None:
+        """q|k|v projection of the quantised input h8, RMSNorm + RoPE, attention, then the attention output quantised per 1x128
+        group and projected by o into `out` (GATE_RES on the residual stream, or BF16 for the self-attention seam)."""
+        C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
+        L = qkv.shape[0]
+        T.begin("gemm_qkv")
+        ops.gemm_fp8(*h8, *b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
+        T.end("gemm_qkv")
+        T.begin("qk_norm_rope")
+        ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, rope_len)
+        T.end("qk_norm_rope")
+        T.begin("self_attention")
+        ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
+        T.end("self_attention")
+        T.begin("gemm_o")
+        a8 = self._act8("att8", L, C)
+        ops.quant_rows_fp8(att, *a8)
+        ops.gemm_fp8(*a8, *b["w_o"], b["b_o"], out, epilogue, gate=gate, tok_idx=tok_idx)
+        T.end("gemm_o")
+
+    def _cross_and_ffn_fp8(self, b, xs, qkv, att, m, tok_idx, ctx) -> None:
+        C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
+        L = xs.shape[0]
+        h8 = self._act8("h8", L, C)
+        ops.ln_modulate_fp8(xs, *h8, None, None, None, b["n3w"], b["n3b"], eps=self.eps)
+        q2 = qkv[:, :C]
+        ops.gemm_fp8(*h8, *b["cw_q"], b["cb_q"], q2, ops.YB_EPI_BF16)
+        ops.rmsnorm_rope(q2, b["cnq"], None, D, self.eps)
+        kv, kvi = ctx
+        T.begin("cross_attention")
+        ops.attention(q2, kv[:, :C], kv[:, C:], att, H)
+        T.end("cross_attention")
+        if kvi is not None:
+            ops.attention(q2, kvi[:, :C], kvi[:, C:], att, H, accumulate=True)
+        a8 = self._act8("att8", L, C)
+        ops.quant_rows_fp8(att, *a8)
+        ops.gemm_fp8(*a8, *b["cw_o"], b["cb_o"], xs, ops.YB_EPI_GATE_RES)
+        ops.ln_modulate_fp8(xs, *h8, m[:, 4], m[:, 3], tok_idx, eps=self.eps)
+        hid8 = self._act8("ffn_hid8", L, self.ffn_dim)
+        T.begin("gemm_ffn1")
+        ops.gemm_fp8(*h8, *b["w1"], b["b1"], hid8[0], ops.YB_EPI_GELU_FP8, out_scale=hid8[1])
+        T.end("gemm_ffn1")
+        T.begin("gemm_ffn2")
+        ops.gemm_fp8(*hid8, *b["w2"], b["b2"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 5], tok_idx=tok_idx)
+        T.end("gemm_ffn2")
+
+    def weight_bytes(self) -> int:
+        """Bytes of every weight tensor the engine holds on its device (bench and tests compare the two precisions)."""
+        seen, total = set(), 0
+
+        def add(t):
+            nonlocal total
+            if isinstance(t, Tensor) and t.data_ptr() not in seen:
+                seen.add(t.data_ptr())
+                total += t.numel() * t.element_size()
+            elif isinstance(t, (tuple, list)):
+                for u in t:
+                    add(u)
+            elif isinstance(t, dict):
+                for u in t.values():
+                    add(u)
+        for v in vars(self).values():
+            if v is self._ws or v is self._rope_cache or v is self._graphs or v is self._ctx_entries:
+                continue
+            add(v)
+        return total
+
     def _cross_kv_one(self, i: int, ctx: Tensor):
         """Block i's cross-attention K | V only (the block / self-attention seams run one block at a time)."""
         C, D = self.dim, self.head_dim
@@ -692,6 +818,9 @@ class WanDiT:
             ctx = self._cross_kv_one(i, context.to(device=self.device, dtype=_BF16).contiguous())
             b = self.blocks[i]
             m = mod[0]
+            if self.precision == "fp8":
+                self._block_fp8(b, xs, m, tok_idx, rope, min(rope_len, L), ctx, L if k_len is None else int(k_len))
+                return xs
             h = self._buf("h", (L, C), _BF16)
             qkv = self._buf("qkv", (L, 3 * C), _BF16)
             att = self._buf("att", (L, C), _BF16)
@@ -714,6 +843,13 @@ class WanDiT:
             rope, rope_len = self.rope_from_reference(freqs, grid, packed)
             qkv = self._buf("qkv", (L, 3 * C), _BF16)
             att = self._buf("att", (L, C), _BF16)
+            if self.precision == "fp8":
+                h8 = self._act8("h8", L, C)
+                ops.quant_rows_fp8(h, *h8)
+                out = torch.empty(L, C, device=self.device, dtype=_BF16)
+                self._self_attention_fp8(b, h8, qkv, att, rope, min(rope_len, L), L if k_len is None else int(k_len), out,
+                                         ops.YB_EPI_BF16)
+                return out
             ops.gemm(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
             ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, min(rope_len, L))
             kl = L if k_len is None else int(k_len)

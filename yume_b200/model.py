@@ -76,19 +76,20 @@ def forward_14b(self, x, t, context, seq_len, clip_fea=None, y=None, rand_num_im
     return out.float(), None
 
 
-def install(model: nn.Module, variant: Optional[str] = None, device="cuda", state_dict=None) -> nn.Module:
+def install(model: nn.Module, variant: Optional[str] = None, device="cuda", state_dict=None, precision: str = "bf16") -> nn.Module:
     """Attach a WanDiT engine to `model` (reference WanModel or the mirrors below) and re-bind its forward.
     Weights are read from the live module at call time (or from `state_dict`, e.g. when the module was built on
-    the meta device); call again after loading a new checkpoint."""
+    the meta device); call again after loading a new checkpoint. precision="fp8" runs the six block linears as e4m3 GEMMs
+    (WanDiT, DESIGN.md §3)."""
     if variant is None:
         variant = "14b" if hasattr(model, "img_emb") else "5b"
     if state_dict is not None:
         model._yb_engine = WanDiT(state_dict, variant, dim=model.dim, ffn_dim=model.ffn_dim, num_heads=model.num_heads,
                                   num_layers=model.num_layers, in_dim=model.in_dim, out_dim=model.out_dim,
                                   text_len=model.text_len, freq_dim=model.freq_dim, patch_size=model.patch_size,
-                                  eps=model.eps, device=device)
+                                  eps=model.eps, device=device, precision=precision)
     else:
-        model._yb_engine = WanDiT.from_module(model, variant, device=device)
+        model._yb_engine = WanDiT.from_module(model, variant, device=device, precision=precision)
     model.forward = types.MethodType(forward_5b if variant == "5b" else forward_14b, model)
     return model
 
@@ -158,8 +159,8 @@ class _WanBase(nn.Module):
         if img:
             self.img_emb = _MLPProj(clip_dim, dim)
 
-    def install(self, device="cuda", state_dict=None):
-        return install(self, self.variant, device, state_dict)
+    def install(self, device="cuda", state_dict=None, precision: str = "bf16"):
+        return install(self, self.variant, device, state_dict, precision=precision)
 
 
 class WanModel5B(_WanBase):

@@ -799,3 +799,91 @@ def vae_unpatchify2_clamp(y: torch.Tensor, out: torch.Tensor, T: int, H: int, W:
           "yb_vae_unpatchify2_clamp")
     _launches += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------
+# FP8 block GEMMs (include/yume_b200_fp8.h). An fp8 activation is a pair: e4m3 values [M, K] and f32 1x128 group scales
+# [K / 128, lds >= M] (group-major).
+# ------------------------------------------------------------------------------------------------------------
+YB_EPI_GELU_FP8 = _lib.YB_EPI_GELU_FP8
+_E4M3 = torch.float8_e4m3fn
+
+
+def fp8_scale_ld(M: int) -> int:
+    """Row stride of an activation-scale table for M rows (the kernels want a multiple of 4)."""
+    return (M + 3) // 4 * 4
+
+
+def gemm_fp8(a: torch.Tensor, a_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor, bias: Optional[torch.Tensor],
+             out: torch.Tensor, epilogue: int, gate: Optional[torch.Tensor] = None, tok_idx: Optional[torch.Tensor] = None,
+             out_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """out = epi(s_w * sum_g s_a[g] * (Aq Wq^T)_g + bias); a e4m3 [M, K] + a_scale f32 [K/128, >= M], w e4m3 [N, K] + w_scale
+    f32 [N]. Epilogues YB_EPI_BF16 / YB_EPI_F32 / YB_EPI_GATE_RES (as gemm) and YB_EPI_GELU_FP8 (out e4m3 + out_scale)."""
+    global _launches, _flops
+    _need(a, _E4M3, "a")
+    _need(w, _E4M3, "w")
+    _need(a_scale, torch.float32, "a_scale")
+    _need(w_scale, torch.float32, "w_scale")
+    M, K = a.shape
+    N, K2 = w.shape
+    if K2 != K:
+        raise YumeB200Error(f"gemm_fp8 K mismatch: {K} vs {K2}")
+    want = {YB_EPI_BF16: torch.bfloat16, YB_EPI_F32: torch.float32, YB_EPI_GATE_RES: torch.float32, YB_EPI_GELU_FP8: _E4M3}
+    if epilogue not in want:
+        raise YumeB200Error(f"gemm_fp8: epilogue {epilogue} is not an fp8 GEMM epilogue")
+    _need(out, want[epilogue], "out")
+    if out.shape[0] != M or out.shape[1] != N:
+        raise YumeB200Error(f"gemm_fp8 out shape {tuple(out.shape)} != ({M}, {N})")
+    if a_scale.shape[0] != K // 128 or w_scale.shape[0] != N:
+        raise YumeB200Error("gemm_fp8: scale tables do not match the operands")
+    for name, t in (("bias", bias), ("gate", gate), ("out_scale", out_scale)):
+        if t is not None:
+            _need(t, torch.float32, name)
+    if tok_idx is not None:
+        _need(tok_idx, torch.int32, "tok_idx")
+    if epilogue == YB_EPI_GELU_FP8 and (out_scale is None or out_scale.shape[0] != N // 128):
+        raise YumeB200Error("gemm_fp8: YB_EPI_GELU_FP8 needs out_scale [N/128, >= M]")
+    args = _lib.GemmFp8Args(
+        struct_bytes=C.sizeof(_lib.GemmFp8Args), M=M, N=N, K=K, A=a.data_ptr(), a_scale=a_scale.data_ptr(), B=w.data_ptr(),
+        b_scale=w_scale.data_ptr(), bias=_ptr(bias), out=out.data_ptr(), out_scale=_ptr(out_scale), gate=_ptr(gate),
+        tok_idx=_ptr(tok_idx), lda=a.stride(0), lds=a_scale.stride(0), ldb=w.stride(0), ldo=out.stride(0),
+        ldos=(out_scale.stride(0) if out_scale is not None else 0), gate_ld=(gate.stride(0) if gate is not None else 0),
+        epilogue=epilogue, block_n=0)
+    check(_lib.load().yb_gemm_fp8(C.byref(args), _stream()), "yb_gemm_fp8")
+    _launches += 1
+    _flops += 2.0 * M * N * K
+    return out
+
+
+def ln_modulate_fp8(x: torch.Tensor, out: torch.Tensor, out_scale: torch.Tensor, scale: Optional[torch.Tensor],
+                    shift: Optional[torch.Tensor], tok_idx: Optional[torch.Tensor] = None, weight: Optional[torch.Tensor] = None,
+                    bias: Optional[torch.Tensor] = None, eps: float = 1e-6) -> torch.Tensor:
+    """ln_modulate with an e4m3 output [L, C] and its 1x128 scales out_scale f32 [C/128, >= L]."""
+    global _launches
+    _need(x, torch.float32, "x")
+    _need(out, _E4M3, "out")
+    _need(out_scale, torch.float32, "out_scale")
+    L, Cdim = x.shape
+    mod_ld = 0
+    for name, t in (("scale", scale), ("shift", shift)):
+        if t is not None:
+            _need(t, torch.float32, name)
+            mod_ld = t.stride(0) if t.dim() == 2 else 0
+    check(_lib.load().yb_ln_modulate_fp8(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), out_scale.data_ptr(),
+                                         out_scale.stride(0), _ptr(scale), _ptr(shift), mod_ld, _ptr(tok_idx), _ptr(weight),
+                                         _ptr(bias), L, Cdim, eps, _stream()), "yb_ln_modulate_fp8")
+    _launches += 1
+    return out
+
+
+def quant_rows_fp8(x: torch.Tensor, out: torch.Tensor, out_scale: torch.Tensor) -> torch.Tensor:
+    """bf16 [M, K] -> e4m3 [M, K] + 1x128 scales out_scale f32 [K/128, >= M]."""
+    global _launches
+    _need(x, torch.bfloat16, "x")
+    _need(out, _E4M3, "out")
+    _need(out_scale, torch.float32, "out_scale")
+    M, K = x.shape
+    check(_lib.load().yb_quant_rows_fp8(x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), out_scale.data_ptr(),
+                                        out_scale.stride(0), M, K, _stream()), "yb_quant_rows_fp8")
+    _launches += 1
+    return out
