@@ -12,6 +12,32 @@
 //   warpgroups 1-2  query rows [64*(wg-1), +64) of the current tile: S = Q K_j^T (wgmma, both operands in smem), masking and
 //                   online softmax on the accumulator fragment, O += P V_j with P as the register A operand
 //
+// Consumer schedule (FlashAttention-3's intra-warpgroup overlap), per query tile of nkv KV tiles:
+//   prologue   issue S_0, wait, softmax(S_0) in place, pack P_0
+//   step j     O *= alpha_j; issue S_{j+1} (not on the last step); issue O += P_j V_j;
+//              wait<1> (S_{j+1} retired) -> softmax(S_{j+1}) in place, while P_j V_j runs on the tensor core;
+//              wait<0> -> pack P_{j+1} (pa / the smem P were P_j V_j's operand until then)
+// Every value goes through the same operations in the same order as a serial schedule (same exp2 arguments, l and O
+// rescaled before the tile's terms are added, same MMA order), so the output is bit-identical to it. The softmax runs in
+// place on S and is packed only after P V retires, so O + S + P = 160 registers are live, not the 224 of keeping S_j and
+// S_{j+1} at once. Variant 1 (P_SMEM, a debug form) shares this schedule. ptxas would otherwise hoist wait<0> above the
+// softmax; a never-taken shared store that depends on l keeps it in place (checked in the SASS: all 66 MUFU.EX2 of a step
+// lie between WARPGROUP.DEPBAR.LE 1 and 0).
+//
+// Barriers (counts are arrivals per phase; the producer and both consumer warpgroups take ring slot it % NS and parity
+// (it / NS) & 1 from one global sequence it: K_j of query tile X at it, V_j at it + 1, 2 nkv positions per tile):
+//   q_full        1 + 32 KB tx  producer arrives; TMA completes      consumers wait, parity X
+//   q_empty       8             each consumer warp once per tile,    producer waits before reloading Q (X = 1)
+//                               after the tile's last S retired
+//   kv_full[s]    1 + 32 KB tx  producer arrives; TMA completes      consumers wait: K_{j+1} before its S, V_j before P V
+//   kv_empty[s]   8             each consumer warp: K_0 after the    producer waits before refilling slot s
+//                               prologue, K_{j+1} after wait<1>,
+//                               V_j after wait<0>
+//   named 1 + wg  128           P_SMEM only: the 4 warps of warpgroup wg, before overwriting and after writing its P
+// A warpgroup holds at most V_j and K_{j+1} (positions it + 1, it + 2) when it waits for K_{j+1}, having released everything
+// up to it; the producer can fill it + 2 once it + 2 - NS <= it is released, so any NS >= 2 is deadlock-free (5 slots, 4 with
+// P_SMEM). Any nkv >= 1 works, so the last, shorter KV segment of the tail split needs nothing special.
+//
 // Tail split: a launch is U = heads x ceil(Lq/256) equal work units. When the last wave is at most half full its T units are each
 // cut into ns KV segments that run as separate CTAs and leave (unnormalised O, row max, row sum) in a workspace; a small combine
 // kernel merges the segments and performs the normal epilogue (bf16 store / Ulysses peer scatter).
@@ -48,9 +74,29 @@ struct AttCfg {
   static constexpr int P_OFF = ATT_TILE_BYTES;   // P_SMEM: 64 x 128 bf16 per consumer warpgroup (2 slabs of 8 KB)
   static constexpr int KV_OFF = P_SMEM ? 2 * ATT_TILE_BYTES : ATT_TILE_BYTES;
   static constexpr int BAR_OFF = KV_OFF + NS * ATT_TILE_BYTES;
+  static constexpr int SINK_OFF = BAR_OFF + 128;   // a word no one reads (see the wait after the softmax)
+  static_assert((2 + 2 * NS) * 8 <= 128, "mbarriers below the sink word");
   static constexpr int SMEM_BYTES = BAR_OFF + 256 + 1024;
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 };
+
+// mbar_wait for the consumer warpgroups: the same bounded wait, but the trap is an asm statement followed by a break
+// instead of the noreturn __trap(). A noreturn call inside the setmaxnreg.inc region makes ptxas allocate the region within
+// the launch's 168 registers rather than 232, and the pipelined loop below then spills.
+__device__ __forceinline__ void att_wait(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > YB_WAIT_LIMIT_CYCLES) {
+#ifdef YB_DEBUG_WAIT
+      printf("yb: attention consumer mbarrier wait timeout block=(%d,%d) thread=%d bar=%u parity=%u\n", blockIdx.x,
+             blockIdx.y, threadIdx.x, smem_u32(bar), parity);
+#endif
+      asm volatile("trap;");
+      break;
+    }
+  }
+}
 
 template <bool P_SMEM>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
@@ -125,34 +171,33 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const float sc = p.scale_log2;
     const uint32_t sQ = smem_u32(smem + Cfg::Q_OFF) + wg * 64 * 128;
     const uint32_t sP = smem_u32(smem + Cfg::P_OFF) + wg * 16384;
+    // S = Q K^T of the K tile at ring position `itk`, committed as one wgmma group and not waited for. s is not zeroed: the
+    // first k-step overwrites it.
+    auto issue_s = [&](float (&s)[64], int itk) {
+      const int slot_k = itk % NS;
+      att_wait(&kv_full[slot_k], (itk / NS) & 1);
+      const uint32_t sK = smem_u32(smem + Cfg::KV_OFF + slot_k * ATT_TILE_BYTES);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 8; ++kk) {   // D = 128: two 64-column slabs, 4 k-steps of 32 B each
+        const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
+        wgmma_ss_acc64<0>(s, make_smem_desc_sw128(sQ + off, 16, 1024), make_smem_desc_sw128(sK + off, 16, 1024), kk != 0);
+      }
+      wgmma_commit();
+    };
     int it = 0;
     for (int X = 0; X < nx; ++X) {
-      mbar_wait(q_full, X);
+      att_wait(q_full, X);
       float o[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) o[i] = 0.f;
       float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;   // rows a / b: running max (log2 domain) and sum
-      for (int j = 0; j < nkv; ++j, it += 2) {
-        const int slot_k = it % NS, slot_v = (it + 1) % NS;
-        mbar_wait(&kv_full[slot_k], (it / NS) & 1);
-        const uint32_t sK = smem_u32(smem + Cfg::KV_OFF + slot_k * ATT_TILE_BYTES);
-        float s[64];
-#pragma unroll
-        for (int i = 0; i < 64; ++i) s[i] = 0.f;
-        wgmma_fence();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {   // D = 128: two 64-column slabs, 4 k-steps of 32 B each
-          const uint32_t off = (kk >> 2) * 16384 + (kk & 3) * 32;
-          wgmma_ss_acc64<0>(s, make_smem_desc_sw128(sQ + off, 16, 1024), make_smem_desc_sw128(sK + off, 16, 1024), kk != 0);
-        }
-        wgmma_commit();
-        wgmma_wait<0>();
-        fence_regs(s);
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&kv_empty[slot_k]);
-          if (j == nkv - 1) mbar_arrive(q_empty);   // the producer may load the next query tile
-        }
+      float al0, al1;      // rescale factors of O for the tile whose P is in pa
+      float s[64];         // S of one KV tile, overwritten in place by its exponentials
+      uint32_t pa[8][4];   // P as the A fragment of the k-steps of P V: k-step kk covers keys [16kk, 16kk + 16)
+      // Online softmax of KV tile j on s: mask, row max, rescale factors, l, and the exponentials in place. O is left to
+      // the caller, which rescales it by al0 / al1 right before the P V of this tile.
+      auto softmax = [&](int j) {
         const int kv_rem = p.Lk - (kv_begin + j) * 128;
         if (kv_rem < 128) {   // last, partial KV tile (k_lens contract): columns past the end count as -inf
 #pragma unroll
@@ -170,33 +215,33 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 1));
         mx1 = fmaxf(mx1, __shfl_xor_sync(0xffffffffu, mx1, 2));
         const float mn0 = fmaxf(m0, mx0 * sc), mn1 = fmaxf(m1, mx1 * sc);
-        const float al0 = fast_exp2(m0 - mn0), al1 = fast_exp2(m1 - mn1);   // 0 on the first tile (m = -inf)
+        al0 = fast_exp2(m0 - mn0);   // 0 on the first tile (m = -inf)
+        al1 = fast_exp2(m1 - mn1);
         m0 = mn0;
         m1 = mn1;
         l0 *= al0;
         l1 *= al1;
 #pragma unroll
-        for (int g = 0; g < 16; ++g) {
-          o[4 * g] *= al0;
-          o[4 * g + 1] *= al0;
-          o[4 * g + 2] *= al1;
-          o[4 * g + 3] *= al1;
-        }
-        // P as the A fragment of the k-steps of P V: k-step kk covers keys [16kk, 16kk + 16) = accumulator groups 2kk, 2kk + 1
-        uint32_t pa[8][4];
+        for (int kk = 0; kk < 8; ++kk) {   // accumulator groups 2kk, 2kk + 1
+          float* e = s + 8 * kk;
 #pragma unroll
-        for (int kk = 0; kk < 8; ++kk) {
-          float e[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) e[i] = fast_exp2(s[8 * kk + i] * sc - ((i & 2) ? m1 : m0));
+          for (int i = 0; i < 8; ++i) e[i] = fast_exp2(e[i] * sc - ((i & 2) ? m1 : m0));
           l0 += (e[0] + e[1]) + (e[4] + e[5]);
           l1 += (e[2] + e[3]) + (e[6] + e[7]);
+        }
+      };
+      // exponentials of s -> bf16 P (registers, or this warpgroup's shared-memory P for variant 1)
+      auto pack_p = [&]() {
+#pragma unroll
+        for (int kk = 0; kk < 8; ++kk) {
+          const float* e = s + 8 * kk;
           pa[kk][0] = pack_bf16x2(e[0], e[1]);   // row a, keys 2t, 2t+1
           pa[kk][1] = pack_bf16x2(e[2], e[3]);   // row b
           pa[kk][2] = pack_bf16x2(e[4], e[5]);   // row a, keys 8 + 2t, +1
           pa[kk][3] = pack_bf16x2(e[6], e[7]);   // row b
         }
         if (P_SMEM) {
+          named_bar_sync(1 + wg, 128);   // every warp's wait for the previous P V is over: P may be overwritten
           // K-major 128B-swizzled P of this warpgroup: slab = key / 64; row r, 16-byte chunk c -> r*128 + ((c ^ (r & 7)) << 4)
           const int ra = row_a - wg * 64, rb = ra + 8;
 #pragma unroll
@@ -211,7 +256,32 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
           fence_proxy_async_smem();
           named_bar_sync(1 + wg, 128);
         }
-        mbar_wait(&kv_full[slot_v], ((it + 1) / NS) & 1);
+      };
+
+      issue_s(s, it);   // prologue: S_0, its softmax and P_0, with nothing to overlap
+      wgmma_wait<0>();
+      fence_regs(s);
+      __syncwarp();
+      if (lane == 0) {
+        mbar_arrive(&kv_empty[it % NS]);
+        if (nkv == 1) mbar_arrive(q_empty);   // that was the tile's last S: the producer may reload Q
+      }
+      softmax(0);
+      pack_p();
+      // KV tile j: P_j is packed and al0 / al1 are its rescale factors (see the schedule in the header). The last tile is a
+      // separate call with next = false so that every wgmma group and wait is unconditional within a call: with a runtime
+      // condition around the S issue and its wait, ptxas serialises every wgmma of the kernel.
+      auto kv_step = [&](int j, const bool next) {
+        const int slot_v = (it + 1) % NS, slot_kn = (it + 2) % NS;
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {   // before the first wgmma of the step: ptxas serialises a stage whose accumulators
+          o[4 * g] *= al0;               // are touched between its wgmmas
+          o[4 * g + 1] *= al0;
+          o[4 * g + 2] *= al1;
+          o[4 * g + 3] *= al1;
+        }
+        if (next) issue_s(s, it + 2);
+        att_wait(&kv_full[slot_v], ((it + 1) / NS) & 1);
         const uint32_t sV = smem_u32(smem + Cfg::KV_OFF + slot_v * ATT_TILE_BYTES);
         wgmma_fence();
 #pragma unroll
@@ -223,11 +293,29 @@ attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
             wgmma_rs_n128_tb(o, pa[kk], vdesc, 1u);
         }
         wgmma_commit();
+        if (next) {
+          wgmma_wait<1>();   // groups retire in order: S_{j+1} is done, P_j V_j may still run
+          fence_regs(s);
+          __syncwarp();
+          if (lane == 0) {
+            mbar_arrive(&kv_empty[slot_kn]);
+            if (j + 2 == nkv) mbar_arrive(q_empty);
+          }
+          softmax(j + 1);
+          // ptxas schedules wgmma.wait_group freely among register arithmetic and would hoist the wait below above the
+          // softmax, leaving nothing to overlap P_j V_j. It keeps the wait after shared-memory accesses, so a store that
+          // depends on every exponential (through l) and is never taken (l >= 0) pins the softmax ahead of the wait.
+          if (l0 + l1 < 0.f) *reinterpret_cast<volatile float*>(smem + Cfg::SINK_OFF) = l0;
+        }
         wgmma_wait<0>();
         fence_regs(o);
         __syncwarp();
         if (lane == 0) mbar_arrive(&kv_empty[slot_v]);
-      }
+        if (next) pack_p();   // pa / the shared-memory P were P_j V_j's operand until now
+        it += 2;
+      };
+      for (int j = 0; j + 1 < nkv; ++j) kv_step(j, true);
+      kv_step(nkv - 1, false);
       l0 += __shfl_xor_sync(0xffffffffu, l0, 1);
       l0 += __shfl_xor_sync(0xffffffffu, l0, 2);
       l1 += __shfl_xor_sync(0xffffffffu, l1, 1);
