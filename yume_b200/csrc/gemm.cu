@@ -16,7 +16,14 @@
 // Structure (one CTA per SM, 384 threads = 3 warpgroups):
 //   warpgroup 0     TMA producer (one thread): A tile 128x64 and B tile block_n x 64 (128B-swizzled) into an smem ring
 //   warpgroups 1-2  consumers: wgmma m64nNk16 over rows [64*(wg-1), +64) of the tile, fp32 accumulators in registers,
-//                   then the fused epilogue (registers -> per-warp smem transpose -> full row segments to global)
+//                   then the fused epilogue, in one of two forms chosen by the launch's output layout:
+//                   - TMA (1-CTA kernel, plain [M, N] output with a 16-byte row pitch: every yb_gemm_bf16 launch except
+//                     RES_BF16 and the N-split layout): each warpgroup writes 64-row x 128-byte boxes of its finished values
+//                     into a swizzled staging buffer and one thread hands each box to the TMA unit as an asynchronous store
+//                     (GATE_RES: a bulk reduce-add into the fp32 residual stream, done in L2), so the next tile's MMAs start
+//                     while the boxes drain;
+//                   - registers -> per-warp smem transpose -> full row segments to global (the SM-pair kernel, the conv
+//                     modes with their scattered voxel rows, the Ulysses layouts, RES_BF16)
 // The SM-pair form (CLUSTER = 2) is a cluster of two CTAs that owns a 256 x block_n tile: each CTA loads its own 128 rows of A
 // and HALF of the B tile, and multicasts that half into both CTAs, so the B operand crosses L2 once per pair of SMs.
 #include "yb_host.h"
@@ -32,7 +39,9 @@ constexpr int GEMM_GROUP_N = 8;   // rasterisation: n-tiles per group (keeps A a
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_SMEM_BYTES = 227 * 1024;                 // the H100 per-block maximum
 constexpr int GEMM_A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
-constexpr int GEMM_EPI_STAGE_BYTES = 8 * 16 * 36 * 4;       // 8 consumer warps x 16 rows x 36 floats
+constexpr int GEMM_EPI_STAGE_BYTES = 8 * 16 * 36 * 4;       // register epilogue: 8 consumer warps x 16 rows x 36 floats
+constexpr int GEMM_EPI_BOX_BYTES = 64 * 128;                // TMA epilogue: one 64-row x 128-byte box (64 bf16 / 32 fp32 columns)
+constexpr int GEMM_EPI_TMA_BYTES = 2 * 2 * GEMM_EPI_BOX_BYTES;   // two staging boxes per consumer warpgroup
 
 struct GemmParams {
   int M, N, K;
@@ -65,6 +74,7 @@ struct GemmParams {
   // for gemm_splitk_combine_kernel. sk_ns == 1: no split (sk_full == number of tiles).
   int sk_full, sk_ns, sk_per;
   float* sk_ws;
+  int tma_out;                  // 1: the epilogue stores through the output tensor map (gemm_has_tma_epilogue instances only)
   // YB_EPI_SP_QKV (internal): the fused q|k|v projection of a Ulysses rank whose epilogue IS the all-to-all — column
   // (part, head h, d) of local token t is stored into the receive buffer of the rank that owns head h (NVLink peer pointer),
   // layout [P(src), Lp, q|k|v of heads/P]; and the per-row sums of squares of the q and k parts (WanRMSNorm spans all heads)
@@ -89,8 +99,20 @@ constexpr int CONVW_A_STAGES = 4;
 __host__ __device__ constexpr int gemm_b_bytes(int block_n) { return ((block_n + 63) / 64) * 64 * GEMM_BLOCK_K * 2; }
 __host__ __device__ constexpr int gemm_stage_bytes(int block_n, int convw) { return (convw ? 0 : GEMM_A_BYTES) + gemm_b_bytes(block_n); }
 __host__ __device__ constexpr int gemm_a_ring_bytes(int convw) { return convw ? CONVW_A_STAGES * CONVW_A_SLAB : 0; }
-static int gemm_stages(int block_n, int convw) {
-  const int s = (GEMM_SMEM_BYTES - 1024 - 256 - GEMM_EPI_STAGE_BYTES - gemm_a_ring_bytes(convw)) / gemm_stage_bytes(block_n, convw);
+// instances that carry the TMA epilogue (the launch still picks it per call through p.tma_out), and their epilogue area: the
+// larger TMA staging area leaves the 256- / 128-wide rings at 4 / 6 stages; the others keep the transpose buffer only
+__host__ __device__ constexpr bool gemm_has_tma_epilogue(int epi, int convw, int cluster) {
+  return cluster == 1 && !convw && (epi == YB_EPI_BF16 || epi == YB_EPI_GELU_BF16 || epi == YB_EPI_GELU_ERF_BF16 ||
+                                    epi == YB_EPI_F32 || epi == YB_EPI_GATE_RES);
+}
+// Of those, GELU / GELU_ERF / GATE_RES only ever write a plain matrix (the conv modes and the N-split layout come with BF16 / F32),
+// so their 1-CTA instances carry no register epilogue at all.
+__host__ __device__ constexpr bool gemm_tma_epilogue_only(int epi, int convw, int cluster) {
+  return gemm_has_tma_epilogue(epi, convw, cluster) && epi != YB_EPI_BF16 && epi != YB_EPI_F32;
+}
+__host__ __device__ constexpr int gemm_epi_bytes(bool tma) { return tma ? GEMM_EPI_TMA_BYTES : GEMM_EPI_STAGE_BYTES; }
+static int gemm_stages(int block_n, int convw, int epi_bytes) {
+  const int s = (GEMM_SMEM_BYTES - 1024 - 256 - epi_bytes - gemm_a_ring_bytes(convw)) / gemm_stage_bytes(block_n, convw);
   return s > GEMM_MAX_STAGES ? GEMM_MAX_STAGES : s;
 }
 
@@ -224,6 +246,89 @@ __device__ __forceinline__ void epilogue_rows16(const GemmParams& p, int col0, i
   }
 }
 
+// TMA epilogue of one consumer warpgroup: its 64 x NM accumulator (rows row0.., columns col0..) leaves as boxes of 64 rows x
+// 128 bytes, 64 bf16 or 32 fp32 columns each. Per box every thread finishes its values in registers (bias, GELU, bf16 rounding;
+// GATE_RES: (acc + bias) * gate[tok[row], col]) and writes them into a staging buffer in the output tensor map's 128B swizzle
+// (16-byte chunk c of box row r at chunk c ^ (r & 7)); one thread then issues the box as a TMA store, or as a bulk reduce-add
+// into the fp32 residual for GATE_RES, and commits it as a bulk group. Two buffers alternate: a buffer is rewritten only after
+// the group that read it two boxes ago has finished reading (wait_group.read 1). `nbox` counts this warpgroup's boxes across
+// tiles so the alternation carries on. Rows past M and columns past N are clipped by the TMA unit.
+template <int EPI, int NM>
+__device__ __forceinline__ void epilogue_tma(const GemmParams& p, const CUtensorMap* tmO, const float (&acc)[128], uint8_t* bufs,
+                                             int row0, int col0, int wg, int wtid, uint32_t& nbox) {
+  constexpr bool kF32 = (EPI == YB_EPI_F32 || EPI == YB_EPI_GATE_RES);
+  constexpr int BOX_COLS = kF32 ? 32 : 64;
+  constexpr int GROUPS = BOX_COLS / 8;   // accumulator column groups of 8 per box
+  if (row0 >= p.M) return;               // uniform over the warpgroup
+  const int lane = wtid & 31;
+  const int r = (wtid >> 5) * 16 + (lane >> 2);   // this thread's box rows r and r + 8 (fragment rows); (r & 7) == lane >> 2
+  const int sw = lane >> 2, c2 = 2 * (lane & 3);
+  const int ncols = min(NM, p.N - col0);
+  const float* g_lo = nullptr;
+  const float* g_hi = nullptr;
+  if (EPI == YB_EPI_GATE_RES && p.gate != nullptr) {
+    int t_lo = 0, t_hi = 0;
+    if (p.tok_idx != nullptr) {
+      if (row0 + r < p.M) t_lo = p.tok_idx[row0 + r];
+      if (row0 + r + 8 < p.M) t_hi = p.tok_idx[row0 + r + 8];
+    }
+    g_lo = p.gate + static_cast<long long>(t_lo) * p.gate_ld;
+    g_hi = p.gate + static_cast<long long>(t_hi) * p.gate_ld;
+  }
+#pragma unroll
+  for (int s = 0; s < NM / BOX_COLS; ++s) {
+    if (s * BOX_COLS < ncols) {
+      uint8_t* buf = bufs + (nbox & 1) * GEMM_EPI_BOX_BYTES;
+      if (wtid == 0) bulk_wait_read<1>();   // the store that last read this buffer is done with it
+      named_bar_sync(1 + wg, 128);
+      // one group of 8 columns at a time (the accumulator of the later boxes is still live): finished values of rows r / r + 8,
+      // columns s * BOX_COLS + 8j + c2, +1
+#pragma unroll
+      for (int j = 0; j < GROUPS; ++j) {
+        const int g = s * GROUPS + j;
+        const int col = col0 + s * BOX_COLS + 8 * j + c2;
+        float2 b = make_float2(0.f, 0.f);
+        const bool in = s * BOX_COLS + 8 * j < ncols;   // N % 32 == 0: a group of 8 columns is all in or all out
+        if (p.bias && in) b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        float2 lo = make_float2(acc[4 * g] + b.x, acc[4 * g + 1] + b.y);
+        float2 hi = make_float2(acc[4 * g + 2] + b.x, acc[4 * g + 3] + b.y);
+        if (EPI == YB_EPI_GELU_BF16) {
+          lo = make_float2(gelu_tanh(lo.x), gelu_tanh(lo.y));
+          hi = make_float2(gelu_tanh(hi.x), gelu_tanh(hi.y));
+        }
+        if (EPI == YB_EPI_GELU_ERF_BF16) {
+          auto ge = [](float v) { return 0.5f * v * (1.0f + erff(v * 0.7071067811865476f)); };
+          lo = make_float2(ge(lo.x), ge(lo.y));
+          hi = make_float2(ge(hi.x), ge(hi.y));
+        }
+        if (EPI == YB_EPI_GATE_RES && g_lo != nullptr && in) {
+          const float2 gl = __ldg(reinterpret_cast<const float2*>(g_lo + col));
+          const float2 gh = __ldg(reinterpret_cast<const float2*>(g_hi + col));
+          lo = make_float2(lo.x * gl.x, lo.y * gl.y);
+          hi = make_float2(hi.x * gh.x, hi.y * gh.y);
+        }
+        if (kF32) {   // 32 bytes per group: chunks 2j, 2j + 1; this pair at byte 8 * (lane & 1) of chunk 2j + (lane & 3) / 2
+          const int off = (((2 * j + ((lane & 3) >> 1)) ^ sw) << 4) + 8 * (lane & 1);
+          *reinterpret_cast<float2*>(buf + r * 128 + off) = lo;
+          *reinterpret_cast<float2*>(buf + (r + 8) * 128 + off) = hi;
+        } else {      // 16 bytes per group: chunk j; this pair at byte 4 * (lane & 3)
+          const int off = ((j ^ sw) << 4) + 4 * (lane & 3);
+          *reinterpret_cast<uint32_t*>(buf + r * 128 + off) = pack_bf16x2(lo.x, lo.y);
+          *reinterpret_cast<uint32_t*>(buf + (r + 8) * 128 + off) = pack_bf16x2(hi.x, hi.y);
+        }
+      }
+      fence_proxy_async_smem();   // make the generic-proxy writes visible to the TMA unit
+      named_bar_sync(1 + wg, 128);
+      if (wtid == 0) {
+        if (EPI == YB_EPI_GATE_RES) tma_reduce_add_2d(tmO, buf, col0 + s * BOX_COLS, row0);
+        else tma_store_2d(tmO, buf, col0 + s * BOX_COLS, row0);
+        bulk_commit();
+      }
+      ++nbox;
+    }
+  }
+}
+
 // one 64-wide K block of this warpgroup's 64 x block_n accumulator: 4 k-steps of 16 (32 B inside the 128-B swizzle row).
 // NM = MMA width: 256 / 128 (block_n equal to it) or 64 (any multiple of 32: block_n / 64 rounded up N = 64 MMAs). A compile-time
 // choice: with the three forms in one kernel ptxas serialises the wgmma pipeline.
@@ -263,15 +368,18 @@ __device__ __forceinline__ void release_slot(uint64_t* bar, int lane) {
 
 template <int EPI, int CONVW, int CLUSTER, int NM>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
+            const GemmParams p) {
   static_assert(!(CONVW && CLUSTER != 1), "the kw-fused conv runs on single CTAs");
+  constexpr bool kTmaEpi = gemm_has_tma_epilogue(EPI, CONVW, CLUSTER);
+  const bool tma_out = gemm_tma_epilogue_only(EPI, CONVW, CLUSTER) || (kTmaEpi && p.tma_out);
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int block_n = p.block_n, stages = p.stages;
   const int stage_bytes = gemm_stage_bytes(block_n, CONVW);
   uint8_t* a_ring = smem + stages * stage_bytes;
   float* epi = reinterpret_cast<float*>(a_ring + gemm_a_ring_bytes(CONVW));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi) + GEMM_EPI_STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(epi) + gemm_epi_bytes(kTmaEpi));
   uint64_t* empty_bar = full_bar + GEMM_MAX_STAGES;
   uint64_t* a_full = empty_bar + GEMM_MAX_STAGES;   // CONVW only
   uint64_t* a_empty = a_full + CONVW_A_STAGES;
@@ -305,6 +413,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if (tma_out) tma_prefetch_desc(&tmO);
     for (int i = 0; i < stages; ++i) {
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8 * CLUSTER);   // every consumer warp of every CTA that writes into the slot
@@ -400,6 +509,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     const int wg = (warp >> 2) - 1;   // rows [64 * wg, +64) of the CTA's 128-row tile
     const int r0 = wg * 64 + (warp & 3) * 16;   // first of the 16 tile rows this warp stores
     float* stage_buf = epi + (warp - 4) * (16 * 36);
+    uint8_t* box_bufs = reinterpret_cast<uint8_t*>(epi) + wg * 2 * GEMM_EPI_BOX_BYTES;   // TMA epilogue: this warpgroup's two boxes
+    uint32_t nbox = 0;
     int stage = 0, a_stage = 0;
     uint32_t phase = 0, a_phase = 0;
     float acc[128];
@@ -410,9 +521,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       decode_work(w, tile, kb0, kb1, part);
       tile_coords(tile, p.num_m_tiles, p.num_n_tiles, m_tile, n_tile);
       const int mt = m_tile * CLUSTER + rank;
-      // logical output row of tile row r0 + (lane & 15): the matrix row, or the voxel index of a conv tile; -1 = none
-      int my_row;
-      {
+      // register epilogue: logical output row of tile row r0 + (lane & 15), the matrix row or the voxel index of a conv tile;
+      // -1 = none
+      int my_row = -1;
+      if (!tma_out) {
         const int r = r0 + (lane & 15);
         if (p.conv) {
           int it, ih, iw;
@@ -507,6 +619,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
         continue;
       }
+      if (tma_out) {
+        epilogue_tma<EPI, NM>(p, &tmO, acc, box_bufs, mt * GEMM_BLOCK_M + wg * 64, n_tile * block_n, wg, threadIdx.x & 127, nbox);
+        continue;
+      }
       int my_tok = 0;  // gate-table row of tile row r0 + lane
       if (EPI == YB_EPI_GATE_RES && p.gate != nullptr && p.tok_idx != nullptr && my_row >= 0) my_tok = p.tok_idx[my_row];
       float sq[2] = {0.f, 0.f};   // SP_QKV: running sum of squares of warp rows it*8 + lane/4 over the current part
@@ -546,6 +662,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
       }
       if (EPI == YB_EPI_SP_QKV) flush_sq(cur_part);
     }
+    if (tma_out && (threadIdx.x & 127) == 0) bulk_wait<0>();   // every box written before the CTA (and its smem) goes away
   }
   if (CLUSTER > 1) cluster_sync_all();   // no CTA leaves while its peer may still multicast into it or arrive on its barriers
 }
@@ -647,10 +764,15 @@ static int pair_max_clusters(Kern kern) {
   return n;
 }
 
-// p.block_n set by the caller; CLUSTER = 2 is the SM-pair form (256-row tiles, multicast B halves)
+// p.block_n set by the caller; CLUSTER = 2 is the SM-pair form (256-row tiles, multicast B halves). tmO: the output tensor map
+// of the TMA epilogue, or null for the register epilogue.
 template <int EPI, int CONVW, int CLUSTER>
-static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams& p, cudaStream_t stream, int split_k = 1,
-                       void* ws = nullptr, long long ws_bytes = 0) {
+static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmO, GemmParams& p, cudaStream_t stream,
+                       int split_k = 1, void* ws = nullptr, long long ws_bytes = 0) {
+  static const CUtensorMap no_map = {};
+  if (gemm_tma_epilogue_only(EPI, CONVW, CLUSTER) && tmO == nullptr) return YB_ERR_ARG;
+  p.tma_out = gemm_has_tma_epilogue(EPI, CONVW, CLUSTER) && tmO != nullptr;
+  if (!p.tma_out) tmO = &no_map;
   // MMA width: the 1-CTA kernel runs 128- and 256-wide tiles only
   const int nm = p.block_n == 256 ? 2 : p.block_n == 128 ? 1 : 0;
   if (CLUSTER == 1 && nm == 0) return YB_ERR_ARG;
@@ -661,7 +783,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   if (CLUSTER == 2) p.num_m_tiles = p.conv ? (p.num_m_tiles + 1) / 2 : (p.M + 255) / 256;   // conv: pairs of 128-voxel boxes
   else if (!p.conv) p.num_m_tiles = (p.M + GEMM_BLOCK_M - 1) / GEMM_BLOCK_M;
   p.num_n_tiles = (p.N + p.block_n - 1) / p.block_n;
-  p.stages = gemm_stages(p.block_n, CONVW);
+  p.stages = gemm_stages(p.block_n, CONVW, gemm_epi_bytes(gemm_has_tma_epilogue(EPI, CONVW, CLUSTER)));
   const int tiles = p.num_m_tiles * p.num_n_tiles;
   // persistent grid: one CTA per SM, or the number of CTA pairs the device holds at once (asked of the driver once per device)
   static int max_clusters[kMaxDevices] = {0};
@@ -693,7 +815,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParam
   attr.val.clusterDim.z = 1;
   cfg.attrs = &attr;
   cfg.numAttrs = 1;
-  (void)cudaLaunchKernelEx(&cfg, kern, tmA, tmB, p);   // a failed launch is reported by check_launch
+  (void)cudaLaunchKernelEx(&cfg, kern, tmA, tmB, *tmO, p);   // a failed launch is reported by check_launch
   int rc = check_launch("gemm");
   if (rc || tail == 0) return rc;
   const long long total = static_cast<long long>(tail) * 256 * (p.block_n / 4);
@@ -758,7 +880,7 @@ extern "C" int yb_gemm_sp_qkv(const void* A, long long lda, const void* W, const
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmB, W, p.N, K, K, p.block_n / 2, GEMM_BLOCK_K);
   if (rc) return rc;
-  return launch_gemm<YB_EPI_SP_QKV, 0, 2>(tmA, tmB, p, reinterpret_cast<cudaStream_t>(stream_));
+  return launch_gemm<YB_EPI_SP_QKV, 0, 2>(tmA, tmB, nullptr, p, reinterpret_cast<cudaStream_t>(stream_));
 }
 
 // Automatic kernel / tile choice of yb_gemm_bf16: the 1-CTA kernel for every shape. On the H100 (700 W) the SM-pair form measured
@@ -861,25 +983,35 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
     rc = make_tmap_bf16_2d(&tmB, a->B, a->N, a->K, a->ldb, bn / 2, GEMM_BLOCK_K);
     if (rc) return rc;
     switch (a->epilogue) {
-      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmB, p, stream);
-      case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 2>(tmA, tmB, p, stream);
-      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmB, p, stream);
-      case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 2>(tmA, tmB, p, stream);
-      case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmB, p, stream);
-      default: return launch_gemm<YB_EPI_GATE_RES, 0, 2>(tmA, tmB, p, stream, a->split_k, a->ws, a->ws_bytes);
+      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmB, nullptr, p, stream);
+      case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 2>(tmA, tmB, nullptr, p, stream);
+      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmB, nullptr, p, stream);
+      case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 2>(tmA, tmB, nullptr, p, stream);
+      case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmB, nullptr, p, stream);
+      default: return launch_gemm<YB_EPI_GATE_RES, 0, 2>(tmA, tmB, nullptr, p, stream, a->split_k, a->ws, a->ws_bytes);
     }
   }
   const int block_n = (a->block_n == 128 || a->block_n == 256) ? a->block_n : ((a->N % 256 == 0 || a->N > 1024) ? 256 : 128);
   rc = make_tmap_bf16_2d(&tmB, a->B, a->N, a->K, a->ldb, block_n, GEMM_BLOCK_K);
   if (rc) return rc;
   p.block_n = block_n;
+  // TMA epilogue for a plain [M, N] output (the row pitch and base were checked above); the N-split layout and RES_BF16 keep the
+  // register epilogue
+  CUtensorMap tmO;
+  const CUtensorMap* tmo = nullptr;
+  if (a->n_split == 0 && a->epilogue != YB_EPI_RES_BF16) {
+    const int elem = (a->epilogue == YB_EPI_F32 || a->epilogue == YB_EPI_GATE_RES) ? 4 : 2;
+    rc = make_tmap_out_2d(&tmO, a->out, a->M, a->N, a->ldo, elem, 64);
+    if (rc) return rc;
+    tmo = &tmO;
+  }
   switch (a->epilogue) {
-    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 1>(tmA, tmB, p, stream);
-    case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 1>(tmA, tmB, p, stream);
-    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 1>(tmA, tmB, p, stream);
-    case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 1>(tmA, tmB, p, stream);
-    case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 1>(tmA, tmB, p, stream);
-    default: return launch_gemm<YB_EPI_GATE_RES, 0, 1>(tmA, tmB, p, stream);
+    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 1>(tmA, tmB, tmo, p, stream);
+    case YB_EPI_GELU_BF16: return launch_gemm<YB_EPI_GELU_BF16, 0, 1>(tmA, tmB, tmo, p, stream);
+    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 1>(tmA, tmB, tmo, p, stream);
+    case YB_EPI_GELU_ERF_BF16: return launch_gemm<YB_EPI_GELU_ERF_BF16, 0, 1>(tmA, tmB, tmo, p, stream);
+    case YB_EPI_RES_BF16: return launch_gemm<YB_EPI_RES_BF16, 0, 1>(tmA, tmB, nullptr, p, stream);
+    default: return launch_gemm<YB_EPI_GATE_RES, 0, 1>(tmA, tmB, tmo, p, stream);
   }
 }
 
@@ -962,17 +1094,17 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
                            p.block_n / 2, GEMM_BLOCK_K);
     if (rc) return rc;
     switch (a->epilogue) {
-      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmBp, p, stream);
-      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmBp, p, stream);
-      default: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmBp, p, stream);
+      case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, 0, 2>(tmA, tmBp, nullptr, p, stream);
+      case YB_EPI_F32: return launch_gemm<YB_EPI_F32, 0, 2>(tmA, tmBp, nullptr, p, stream);
+      default: return launch_gemm<YB_EPI_RES_BF16, 0, 2>(tmA, tmBp, nullptr, p, stream);
     }
   }
   p.block_n = block_n;
 #define YB_CONV_DISPATCH(CW)                                                                  \
   switch (a->epilogue) {                                                                     \
-    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, CW, 1>(tmA, tmB, p, stream);            \
-    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, CW, 1>(tmA, tmB, p, stream);              \
-    default: return launch_gemm<YB_EPI_RES_BF16, CW, 1>(tmA, tmB, p, stream);                 \
+    case YB_EPI_BF16: return launch_gemm<YB_EPI_BF16, CW, 1>(tmA, tmB, nullptr, p, stream);   \
+    case YB_EPI_F32: return launch_gemm<YB_EPI_F32, CW, 1>(tmA, tmB, nullptr, p, stream);     \
+    default: return launch_gemm<YB_EPI_RES_BF16, CW, 1>(tmA, tmB, nullptr, p, stream);        \
   }
   if (fuse_w) {
     YB_CONV_DISPATCH(1)

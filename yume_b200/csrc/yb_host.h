@@ -45,6 +45,24 @@ inline int make_tmap_bf16_2d(CUtensorMap* tm, const void* base, uint64_t rows, u
   return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
 }
 
+// 2D output tensor map (bf16 or fp32, `elem_bytes` 2 / 4) for TMA stores and reduce-adds: global view [rows, cols] with row
+// stride `ld` elements, boxes of box_rows x 128 bytes, 128-byte swizzle. Writes outside [rows, cols] are dropped, so a view
+// narrower than its buffer (ld > cols) leaves the columns past `cols` untouched.
+inline int make_tmap_out_2d(CUtensorMap* tm, void* base, uint64_t rows, uint64_t cols, uint64_t ld, int elem_bytes,
+                            uint32_t box_rows) {
+  PFN_encodeTiled fn = get_encode_fn();
+  if (!fn) return YB_ERR_NO_DRIVER;
+  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || ((ld * elem_bytes) & 0xF)) return YB_ERR_ALIGNMENT;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstride[1] = {ld * elem_bytes};
+  cuuint32_t box[2] = {static_cast<cuuint32_t>(128 / elem_bytes), box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(tm, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, base, gdim, gstride,
+                  box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
+}
+
 // 3D bf16 tensor map: [chunks, rows, cols] with row stride `ld` and chunk stride `chunk_ld` (elements),
 // box {box_cols, box_rows, 1}. Used for a K-split A operand: logical column k = chunk * cols + c.
 inline int make_tmap_bf16_3d(CUtensorMap* tm, const void* base, uint64_t chunks, uint64_t rows, uint64_t cols,

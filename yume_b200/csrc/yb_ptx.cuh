@@ -1,5 +1,5 @@
-// yb_ptx.cuh — thin inline-PTX wrappers for sm_90a (H100): mbarrier, TMA (cp.async.bulk.tensor, with cluster
-// multicast), cluster barriers / remote mbarrier arrivals, wgmma (warpgroup MMA) and its shared-memory descriptors.
+// yb_ptx.cuh — thin inline-PTX wrappers for sm_90a (H100): mbarrier, TMA (cp.async.bulk.tensor loads with cluster multicast,
+// stores and reduce-adds), cluster barriers / remote mbarrier arrivals, wgmma (warpgroup MMA) and its shared-memory descriptors.
 // Everything here is hand-written for sm_90a; there is no fallback path for other architectures.
 #pragma once
 #include <cstdint>
@@ -149,6 +149,30 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* t
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2),
       "r"(c3)
       : "memory");
+}
+// 2D tiled store of a shared-memory box to global memory, and its reduce-add form (the L2 adds the box into what global
+// memory holds; the element type is the tensor map's). Out-of-range rows and columns of the box are not written. Both join the
+// issuing thread's current bulk group.
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* tmap, const void* smem_src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() {
+  asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory");
+}
+// at most N of this thread's bulk groups not yet complete (their global writes done)
+template <int N>
+__device__ __forceinline__ void bulk_wait() {
+  asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
 // ----------------------------------------------------------------------------------------------
