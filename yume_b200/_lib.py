@@ -145,6 +145,12 @@ FP8_SIGNATURES = {
     "yb_quant_rows_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
 }
 
+# every symbol include/yume_b200_fp8_attn.h declares (the e4m3 self-attention of precision="fp8_attn")
+FP8_ATTN_SIGNATURES = {
+    "yb_quant_vt_fp8": (_i, [_vp, _ll, _vp, _vp, _i, _i, _vp]),
+    "yb_attention_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _f, _i, _vp, _ll, _vp]),
+}
+
 _lib = None
 
 
@@ -166,7 +172,7 @@ def load():
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
-                              **FP8_SIGNATURES}.items():
+                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

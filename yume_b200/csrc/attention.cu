@@ -456,6 +456,23 @@ static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, cons
   return check_launch("attention_combine");
 }
 
+// the combine for another attention kernel that writes its KV-segment partials in this layout (attention_fp8.cu)
+int attention_combine_launch(void* out, long long ldo, int Lq, int nq, int full_units, int ns, int tail, float* ws_o,
+                             float* ws_ml, cudaStream_t stream) {
+  AttParams p = {};
+  p.out = static_cast<__nv_bfloat16*>(out);
+  p.ldo = ldo;
+  p.Lq = Lq;
+  p.sp_world = 1;
+  p.nq = nq;
+  p.full_units = full_units;
+  p.ns = ns;
+  p.ws_o = ws_o;
+  p.ws_ml = ws_ml;
+  attention_combine_kernel<<<tail * 32, 256, 0, stream>>>(p, tail);
+  return check_launch("attention_combine");
+}
+
 // debug variant (P through shared memory) selected by flags bit 0
 static int dispatch_attention(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv,
                               AttParams p, int heads, cudaStream_t stream, int flags, void* ws, long long ws_bytes) {

@@ -108,6 +108,11 @@ inline int check_launch(const char* what) {
   return YB_OK;
 }
 
+// attention.cu: merge the KV-segment partials (O in true units [tail * ns, 256, 128], then (row max log2, row sum)
+// [tail * ns, 256, 2]) of the `tail` units after the first `full_units` and store bf16 rows of out (see yb_attention_plan)
+int attention_combine_launch(void* out, long long ldo, int Lq, int nq, int full_units, int ns, int tail, float* ws_o,
+                             float* ws_ml, cudaStream_t stream);
+
 constexpr int kMaxDevices = 64;
 inline int current_device() {
   int dev = 0;

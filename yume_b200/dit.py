@@ -108,6 +108,7 @@ def framepack_plan(hist: int, branch_hist: int) -> List[_Segment]:
 FP8_MAX = 448.0                                  # largest finite e4m3 value
 FP8_WEIGHTS = ("w_qkv", "w_o", "cw_q", "cw_o", "w1", "w2")   # the block linears that precision="fp8" converts
 FP8_LN_WIDTHS = (256, 1024, 3072, 5120)          # model widths yb_ln_modulate_fp8 has an instance for
+PRECISIONS = ("bf16", "fp8", "fp8_attn")         # WanDiT(precision=): see WanDiT.__init__
 
 
 def quantize_weight_fp8(w: Tensor) -> Tuple[Tensor, Tensor]:
@@ -144,12 +145,13 @@ class WanDiT:
                  precision: str = "bf16"):
         if variant not in ("5b", "14b"):
             raise YumeB200Error("variant must be '5b' or '14b'")
-        if precision not in ("bf16", "fp8"):
-            raise YumeB200Error("precision must be 'bf16' or 'fp8'")
-        if precision == "fp8" and (dim % 128 or ffn_dim % 128):
-            raise YumeB200Error(f"precision='fp8' needs dim and ffn_dim divisible by 128 (1x128 scale groups), got {dim}, {ffn_dim}")
-        if precision == "fp8" and dim not in FP8_LN_WIDTHS:
-            raise YumeB200Error(f"precision='fp8' runs the fp8 LayerNorm at dim {FP8_LN_WIDTHS} only, got {dim}")
+        if precision not in PRECISIONS:
+            raise YumeB200Error("precision must be 'bf16', 'fp8' or 'fp8_attn'")
+        if precision != "bf16" and (dim % 128 or ffn_dim % 128):
+            raise YumeB200Error(f"precision={precision!r} needs dim and ffn_dim divisible by 128 (1x128 scale groups), got {dim}, "
+                                f"{ffn_dim}")
+        if precision != "bf16" and dim not in FP8_LN_WIDTHS:
+            raise YumeB200Error(f"precision={precision!r} runs the fp8 LayerNorm at dim {FP8_LN_WIDTHS} only, got {dim}")
         if tuple(patch_size) != (1, 2, 2):
             raise YumeB200Error("only patch_size (1, 2, 2) is supported (both Yume models use it)")
         if dim % num_heads or dim // num_heads != 128:
@@ -159,8 +161,10 @@ class WanDiT:
         self.device = torch.device(device)
         self.head_dim = 128
         # "fp8": the six block linears (q|k|v, o, cross q, cross o, ffn.0, ffn.2) run as e4m3 GEMMs with per-channel weight
-        # scales and 1x128 activation scales (include/yume_b200_fp8.h); everything else stays as in "bf16"
+        # scales and 1x128 activation scales (include/yume_b200_fp8.h); everything else stays as in "bf16".
+        # "fp8_attn": everything "fp8" does, and the self-attention of every block in e4m3 (include/yume_b200_fp8_attn.h)
         self.precision = precision
+        self._fp8 = precision != "bf16"
         self._ws: Dict[Tuple, Tensor] = {}
         self._rope_cache: Dict[Tuple, Tensor] = {}
         self.timer = KernelTimer()          # bench.py switches it on to time individual kernels inside a live step
@@ -265,7 +269,7 @@ class WanDiT:
         exactly the chunks the all-to-all sends."""
         if transport not in ("auto", "p2p", "p2p_gemm", "nccl"):
             raise YumeB200Error("transport must be auto, p2p, p2p_gemm or nccl")
-        if self.precision == "fp8":
+        if self._fp8:
             raise YumeB200Error("sequence parallelism runs the bf16 block GEMMs only: build the engine with precision='bf16'")
         self.sp_transport, self._sp_p2p = transport, None
         import torch.distributed as dist
@@ -616,7 +620,7 @@ class WanDiT:
     def _block(self, i: int, xs: Tensor, mod: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int,
                ctx: Tensor, L_true: Optional[int] = None) -> None:
         """One WanAttentionBlock in place on the fp32 residual stream xs [L, C] (a token shard under Ulysses)."""
-        if self.precision == "fp8":
+        if self._fp8:
             return self._block_fp8(self.blocks[i], xs, mod[i], tok_idx, rope, rope_len,
                                    ctx[i] if isinstance(ctx, list) else self._cross_kv(ctx)[i],
                                    L_true if L_true is not None else xs.shape[0])
@@ -648,7 +652,10 @@ class WanDiT:
         ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, rope_len)
         T.end("qk_norm_rope")
         T.begin("self_attention")
-        ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
+        if self.precision == "fp8_attn":
+            self._attention_fp8(qkv, att, k_len)
+        else:
+            ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
         T.end("self_attention")
         T.begin("gemm_o")
         ops.gemm(att, b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
@@ -714,13 +721,30 @@ class WanDiT:
         ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, rope_len)
         T.end("qk_norm_rope")
         T.begin("self_attention")
-        ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
+        if self.precision == "fp8_attn":
+            self._attention_fp8(qkv, att, k_len)
+        else:
+            ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
         T.end("self_attention")
         T.begin("gemm_o")
         a8 = self._act8("att8", L, C)
         ops.quant_rows_fp8(att, *a8)
         ops.gemm_fp8(*a8, *b["w_o"], b["b_o"], out, epilogue, gate=gate, tok_idx=tok_idx)
         T.end("gemm_o")
+
+    def _attention_fp8(self, qkv: Tensor, att: Tensor, k_len: int) -> None:
+        """precision="fp8_attn": self-attention of the normed, roped q|k|v rows on e4m3 operands (include/yume_b200_fp8_attn.h).
+        q and k are quantised by one launch over the [L, 2C] view (a 1x128 group is one head of one token: q scales of head h
+        at scale row h, k scales at heads + h), v transposed per (head, 128-key tile); out bf16 `att`."""
+        C, H = self.dim, self.heads
+        L = qkv.shape[0]
+        Lkp = ops.vt8_keys(k_len)
+        qk8, qk_s = self._act8("qk8", L, 2 * C)
+        vt8 = self._buf("vt8", (H, 128, Lkp), torch.float8_e4m3fn)
+        v_s = self._buf("vt8_s", (H, Lkp // 128), _F32)
+        ops.quant_rows_fp8(qkv[:, :2 * C], qk8, qk_s)
+        ops.quant_vt_fp8(qkv[:k_len, 2 * C:], vt8, v_s, H)
+        ops.attention_fp8(qk8[:, :C], qk8[:k_len, C:], qk_s, vt8, v_s, att, H)
 
     def _cross_and_ffn_fp8(self, b, xs, qkv, att, m, tok_idx, ctx) -> None:
         C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
@@ -818,7 +842,7 @@ class WanDiT:
             ctx = self._cross_kv_one(i, context.to(device=self.device, dtype=_BF16).contiguous())
             b = self.blocks[i]
             m = mod[0]
-            if self.precision == "fp8":
+            if self._fp8:
                 self._block_fp8(b, xs, m, tok_idx, rope, min(rope_len, L), ctx, L if k_len is None else int(k_len))
                 return xs
             h = self._buf("h", (L, C), _BF16)
@@ -843,7 +867,7 @@ class WanDiT:
             rope, rope_len = self.rope_from_reference(freqs, grid, packed)
             qkv = self._buf("qkv", (L, 3 * C), _BF16)
             att = self._buf("att", (L, C), _BF16)
-            if self.precision == "fp8":
+            if self._fp8:
                 h8 = self._act8("h8", L, C)
                 ops.quant_rows_fp8(h, *h8)
                 out = torch.empty(L, C, device=self.device, dtype=_BF16)

@@ -79,8 +79,8 @@ def forward_14b(self, x, t, context, seq_len, clip_fea=None, y=None, rand_num_im
 def install(model: nn.Module, variant: Optional[str] = None, device="cuda", state_dict=None, precision: str = "bf16") -> nn.Module:
     """Attach a WanDiT engine to `model` (reference WanModel or the mirrors below) and re-bind its forward.
     Weights are read from the live module at call time (or from `state_dict`, e.g. when the module was built on
-    the meta device); call again after loading a new checkpoint. precision="fp8" runs the six block linears as e4m3 GEMMs
-    (WanDiT, DESIGN.md §3)."""
+    the meta device); call again after loading a new checkpoint. precision="fp8" runs the six block linears as e4m3 GEMMs,
+    precision="fp8_attn" also the self-attention (WanDiT, DESIGN.md §3)."""
     if variant is None:
         variant = "14b" if hasattr(model, "img_emb") else "5b"
     if state_dict is not None:

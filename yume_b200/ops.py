@@ -887,3 +887,64 @@ def quant_rows_fp8(x: torch.Tensor, out: torch.Tensor, out_scale: torch.Tensor) 
                                         out_scale.stride(0), M, K, _stream()), "yb_quant_rows_fp8")
     _launches += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------
+# FP8 self-attention (include/yume_b200_fp8_attn.h): q and k quantised per (token, head) by quant_rows_fp8 over the [L, 2C]
+# view of the fused q|k|v rows, v by quant_vt_fp8 per (head, 128-key tile) into the transposed, key-permuted vt8.
+# ------------------------------------------------------------------------------------------------------------
+def vt8_keys(Lk: int) -> int:
+    """Key columns of vt8 for Lk keys: Lk rounded up to whole 128-key tiles."""
+    return (Lk + 127) // 128 * 128
+
+
+def quant_vt_fp8(v: torch.Tensor, vt8: torch.Tensor, v_scale: torch.Tensor, heads: int) -> torch.Tensor:
+    """v bf16 [Lk, heads*128] (row stride % 8) -> vt8 e4m3 [heads, 128, Lkp] + v_scale f32 [heads, Lkp/128]."""
+    global _launches
+    _need(v, torch.bfloat16, "v")
+    _need(vt8, _E4M3, "vt8")
+    _need(v_scale, torch.float32, "v_scale")
+    Lk = v.shape[0]
+    Lkp = vt8_keys(Lk)
+    if v.shape[1] != heads * 128:
+        raise YumeB200Error("quant_vt_fp8 supports head_dim 128 only")
+    if tuple(vt8.shape) != (heads, 128, Lkp) or not vt8.is_contiguous():
+        raise YumeB200Error(f"quant_vt_fp8: vt8 must be contiguous [{heads}, 128, {Lkp}], got {tuple(vt8.shape)}")
+    if tuple(v_scale.shape) != (heads, Lkp // 128) or not v_scale.is_contiguous():
+        raise YumeB200Error(f"quant_vt_fp8: v_scale must be contiguous [{heads}, {Lkp // 128}], got {tuple(v_scale.shape)}")
+    check(_lib.load().yb_quant_vt_fp8(v.data_ptr(), v.stride(0), vt8.data_ptr(), v_scale.data_ptr(), Lk, heads, _stream()),
+          "yb_quant_vt_fp8")
+    _launches += 1
+    return vt8
+
+
+def attention_fp8(q8: torch.Tensor, k8: torch.Tensor, qk_scale: torch.Tensor, vt8: torch.Tensor, v_scale: torch.Tensor,
+                  out: torch.Tensor, heads: int, scale: Optional[float] = None, split: int = 0) -> torch.Tensor:
+    """softmax(q k^T * scale) v on e4m3 operands, non-causal. q8 [Lq, heads*128], k8 [Lk, heads*128] e4m3 (row strides % 16),
+    qk_scale f32 [2*heads, >= max(Lq, Lk)] (q scales, then k scales), vt8 / v_scale as quant_vt_fp8 wrote them for Lk keys,
+    out bf16 [Lq, heads*128]. split: KV split policy as for attention."""
+    global _launches, _flops
+    _need(q8, _E4M3, "q8")
+    _need(k8, _E4M3, "k8")
+    _need(qk_scale, torch.float32, "qk_scale")
+    _need(vt8, _E4M3, "vt8")
+    _need(v_scale, torch.float32, "v_scale")
+    _need(out, torch.bfloat16, "out")
+    Lq, Lk = q8.shape[0], k8.shape[0]
+    Lkp = vt8_keys(Lk)
+    if q8.shape[1] != heads * 128 or k8.shape[1] != heads * 128 or out.shape[1] != heads * 128 or out.shape[0] != Lq:
+        raise YumeB200Error("attention_fp8 supports head_dim 128 only, with out [Lq, heads*128]")
+    if qk_scale.shape[0] != 2 * heads:
+        raise YumeB200Error(f"attention_fp8: qk_scale must have {2 * heads} rows (q scales, then k scales)")
+    if tuple(vt8.shape) != (heads, 128, Lkp) or tuple(v_scale.shape) != (heads, Lkp // 128):
+        raise YumeB200Error("attention_fp8: vt8 / v_scale do not match Lk and heads")
+    if scale is None:
+        scale = 1.0 / math.sqrt(128.0)
+    flags = (split & 7) << 4
+    ws, ws_bytes = _attention_ws(Lq, Lk, heads, flags, q8.device)
+    check(_lib.load().yb_attention_fp8(q8.data_ptr(), q8.stride(0), k8.data_ptr(), k8.stride(0), qk_scale.data_ptr(),
+                                       qk_scale.stride(0), vt8.data_ptr(), v_scale.data_ptr(), out.data_ptr(), out.stride(0), Lq,
+                                       Lk, heads, scale, flags, _ptr(ws), ws_bytes, _stream()), "yb_attention_fp8")
+    _launches += 1
+    _flops += 4.0 * Lq * Lk * heads * 128
+    return out
