@@ -151,6 +151,23 @@ FP8_ATTN_SIGNATURES = {
     "yb_attention_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _f, _i, _vp, _ll, _vp]),
 }
 
+# every symbol include/yume_b200_fp8_vae.h declares (the e4m3 convs of Wan22VaeDecoder(precision="fp8"))
+class Conv3dFp8Args(C.Structure):
+    """Mirror of `struct yb_conv3d_fp8_args` (include/yume_b200_fp8_vae.h)."""
+
+    _fields_ = [
+        ("struct_bytes", C.c_uint), ("x", C.c_void_p), ("x_scale", C.c_void_p), ("w", C.c_void_p), ("w_scale", C.c_void_p),
+        ("bias", C.c_void_p), ("out", C.c_void_p), ("res", C.c_void_p), ("ldo", C.c_longlong), ("res_ld", C.c_longlong),
+        ("T", C.c_int), ("H", C.c_int), ("W", C.c_int), ("Cp", C.c_int), ("Cout", C.c_int),
+        ("kt", C.c_int), ("kh", C.c_int), ("kw", C.c_int), ("t_hist", C.c_int), ("epilogue", C.c_int),
+    ]
+
+
+FP8_VAE_SIGNATURES = {
+    "yb_conv3d_fp8": (_i, [C.POINTER(Conv3dFp8Args), _vp]),
+    "yb_vae_rms_act_fp8": (_i, [_vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+}
+
 _lib = None
 
 
@@ -172,7 +189,7 @@ def load():
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
-                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES}.items():
+                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

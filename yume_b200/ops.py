@@ -948,3 +948,56 @@ def attention_fp8(q8: torch.Tensor, k8: torch.Tensor, qk_scale: torch.Tensor, vt
     _launches += 1
     _flops += 4.0 * Lq * Lk * heads * 128
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------
+# FP8 Wan2.2 VAE decode convs (include/yume_b200_fp8_vae.h). An fp8 activation stream is a pair: e4m3 values [T, H, W, Cp] and
+# f32 scales [T, Cp / 128, H, W], one per voxel and 128-channel group (frame-major: a frame of both is one contiguous block).
+# ------------------------------------------------------------------------------------------------------------
+def vae_rms_act_fp8(x: torch.Tensor, dims, out: torch.Tensor, out_scale: torch.Tensor, gamma: Optional[torch.Tensor], up: int = 1,
+                    silu: bool = True) -> torch.Tensor:
+    """vae_rms_act with an e4m3 output: x bf16 [T*Hs*Ws, C] -> out e4m3 [T, Hs*up, Ws*up, Cp] + out_scale f32
+    [T, Cp/128, Hs*up, Ws*up] (both contiguous), the quantisation of the bf16 values vae_rms_act writes."""
+    global _launches
+    _need(x, torch.bfloat16, "x")
+    _need(out, _E4M3, "out")
+    _need(out_scale, torch.float32, "out_scale")
+    T, Hs, Ws = dims
+    Cp = out.shape[-1]
+    if not (out.is_contiguous() and out_scale.is_contiguous()) or \
+            tuple(out_scale.shape) != (out.shape[0], Cp // 128, out.shape[1], out.shape[2]):
+        raise YumeB200Error("vae_rms_act_fp8: out [T, H, W, Cp] and out_scale [T, Cp/128, H, W] must be contiguous and match")
+    check(_lib.load().yb_vae_rms_act_fp8(x.data_ptr(), x.stride(0), out.data_ptr(), out_scale.data_ptr(), _ptr(gamma), T, Hs, Ws,
+                                         x.shape[1], Cp, up, 1 if silu else 0, _stream()), "yb_vae_rms_act_fp8")
+    _launches += 1
+    return out
+
+
+def conv3d_fp8(x: torch.Tensor, x_scale: torch.Tensor, w: torch.Tensor, w_scale: torch.Tensor, bias: Optional[torch.Tensor],
+               out: torch.Tensor, T: int, H: int, W: int, t_hist: int = 0, epilogue: int = YB_EPI_BF16,
+               res: Optional[torch.Tensor] = None, taps=(3, 3, 3)) -> torch.Tensor:
+    """Zero-padded causal conv with e4m3 operands: x e4m3 [t_hist + T, H, W, Cp] + x_scale f32 [t_hist + T, Cp/128, H, W]
+    (t_hist = 0, or kt - 1 carried frames in front), w e4m3 [Cout, taps*Cp] + w_scale f32 [Cout] -> out bf16 [T*H*W, >= Cout]
+    (YB_EPI_BF16, or YB_EPI_RES_BF16 with res)."""
+    global _launches, _flops
+    _need(x, _E4M3, "x")
+    _need(x_scale, torch.float32, "x_scale")
+    _need(w, _E4M3, "w")
+    _need(w_scale, torch.float32, "w_scale")
+    _need(out, torch.bfloat16, "out")
+    if res is not None:
+        _need(res, torch.bfloat16, "res")
+    kt, kh, kw = taps
+    Cp = x.shape[-1]
+    if tuple(x.shape[:3]) != (t_hist + T, H, W) or not x.is_contiguous() or not x_scale.is_contiguous() or \
+            tuple(x_scale.shape) != (t_hist + T, Cp // 128, H, W) or w.shape[1] != kt * kh * kw * Cp or not w.is_contiguous():
+        raise YumeB200Error("conv3d_fp8: bad input / scale / weight layout")
+    args = _lib.Conv3dFp8Args(
+        struct_bytes=C.sizeof(_lib.Conv3dFp8Args), x=x.data_ptr(), x_scale=x_scale.data_ptr(), w=w.data_ptr(),
+        w_scale=w_scale.data_ptr(), bias=_ptr(bias), out=out.data_ptr(), res=_ptr(res), ldo=out.stride(0),
+        res_ld=(res.stride(0) if res is not None else 0), T=T, H=H, W=W, Cp=Cp, Cout=w.shape[0], kt=kt, kh=kh, kw=kw,
+        t_hist=t_hist, epilogue=epilogue)
+    check(_lib.load().yb_conv3d_fp8(C.byref(args), _stream()), "yb_conv3d_fp8")
+    _launches += 1
+    _flops += 2.0 * T * H * W * kt * kh * kw * Cp * w.shape[0]
+    return out

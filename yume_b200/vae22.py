@@ -34,6 +34,7 @@ import torch
 
 from . import ops
 from ._lib import YumeB200Error
+from .dit import quantize_weight_fp8
 from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _rup, chunk_lengths  # noqa: F401  (chunk_lengths: re-exported)
 
 Tensor = torch.Tensor
@@ -148,7 +149,7 @@ class WanVaeDecoder(WanVaeEngine):
                 x, T = y, y.shape[0] // HW
             else:
                 self._keep(key, self._new(0, H, W, _rup(C, 64)))
-        a = self._act(x, (T, H, W), None, False, up=2)           # nearest-exact 2x, then Conv2d 3x3 (zero pad 1)
+        a = self._act(x, (T, H, W), None, False, up=2, conv=p + ".resample.1")   # nearest-exact 2x, then Conv2d 3x3 (zero pad 1)
         return self._conv(p + ".resample.1", a, (T, 2 * H, 2 * W)), (T, 2 * H, 2 * W)
 
     def _head(self, L: Layer, x: Tensor, dims, out: Tensor) -> None:
@@ -182,13 +183,27 @@ class WanVaeDecoder(WanVaeEngine):
         return self._plan(T, lambda n: self.chunk_bytes(n, T, H, W))
 
 
+FP8_CONV_SUFFIXES = (".residual.2", ".residual.6", ".resample.1")
+
+
+def fp8_conv(name: str, cp: int, cout: int) -> bool:
+    """The per-conv rule of Wan22VaeDecoder(precision="fp8"): the res-block convs and the Resample Conv2d run on e4m3 operands
+    when the padded input width cp and the packed output width cout are multiples of 128 (whole 128-channel scale groups and
+    128-wide output tiles). decoder.conv1 (cp 64), the time_convs (their input is a conv output, not a quantising norm pass),
+    the 1x1 shortcuts, the mid attention and the head stay bf16."""
+    return name.endswith(FP8_CONV_SUFFIXES) and cp % 128 == 0 and cout % 128 == 0
+
+
 class Wan22VaeDecoder(WanVaeDecoder):
-    """`Wan2_2_VAE.decode` (vae2_2.py:1059-1072): z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 16H, 16W]."""
+    """`Wan2_2_VAE.decode` (vae2_2.py:1059-1072): z [z_dim, T, H, W] -> f32 [3, 4(T-1)+1, 16H, 16W].
+    precision="fp8" runs the convs `fp8_conv` selects on e4m3 operands (include/yume_b200_fp8_vae.h); "bf16" (the default)
+    runs every layer in bf16."""
     SCALE = 16                                                   # three 2x spatial upsamples, then unpatchify 2x
+    PRECISIONS = ("bf16", "fp8")
 
     def __init__(self, sd: Dict[str, Tensor], dec_dim: int = 256, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_upsample: Sequence[bool] = (True, True, False),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
         self.dims = dims = [dec_dim * u for u in [dim_mult[-1]] + list(dim_mult[::-1])]      # vae2_2.py:656
         layers = decoder_front(dims[0])
         for i in range(len(dim_mult)):                           # Up_ResidualBlock (:461-503)
@@ -201,7 +216,18 @@ class Wan22VaeDecoder(WanVaeDecoder):
                 ft = 2 if i < len(temperal_upsample) and temperal_upsample[i] else 1
                 layers += [Layer("up", f"{p}.{num_res_blocks + 1}", co, co, ft, 2), Layer("dupup", ci=ci, co=co, ft=ft, fs=2)]
         layers.append(Layer("head", "decoder.head.2", dims[-1], _rup(12, 32)))
-        super().__init__(sd, z_dim, layers, mean, std, device)
+        super().__init__(sd, z_dim, layers, mean, std, device, precision)
+
+    def _repack(self, sd: Dict[str, Tensor], mean: Tensor, std: Tensor) -> None:
+        super()._repack(sd, mean, std)
+        self.conv8 = {}
+        if self.precision != "fp8":
+            return
+        for name, (w, b, taps) in list(self.conv.items()):
+            if fp8_conv(name, w.shape[1] // math.prod(taps), w.shape[0]):
+                wq, sw = quantize_weight_fp8(w)                  # per output channel over taps x cp, from the packed bf16 weight
+                self.conv8[name] = (wq, sw, b, taps)
+                del self.conv[name]                              # no bf16 copy of a converted weight is kept
 
     def _write(self, y: Tensor, out: Tensor, dims) -> None:
         if self._one_pass:
@@ -210,9 +236,9 @@ class Wan22VaeDecoder(WanVaeDecoder):
             ops.vae_unpatchify2_clamp_win(y, out, *dims)
 
 
-def install_wan22_vae(vae, device="cuda"):
+def install_wan22_vae(vae, device="cuda", precision: str = "bf16"):
     """Attach a Wan22VaeDecoder to a live reference `Wan2_2_VAE` wrapper and re-bind its `decode(zs)` (same list-in /
-    list-out contract and TypeError behaviour as vae2_2.py:1059-1072)."""
+    list-out contract and TypeError behaviour as vae2_2.py:1059-1072). precision: see Wan22VaeDecoder."""
     m = vae.model
     sd = dict(m.state_dict())
     dims0 = sd["decoder.conv1.weight"].shape[0]
@@ -220,7 +246,8 @@ def install_wan22_vae(vae, device="cuda"):
     mean, inv_std = vae.scale
     eng = Wan22VaeDecoder(sd, dec_dim=dims0 // dim_mult[-1], z_dim=m.z_dim, dim_mult=dim_mult,
                           num_res_blocks=m.num_res_blocks, temperal_upsample=m.temperal_upsample,
-                          mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device)
+                          mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device,
+                          precision=precision)
     vae._yb_decoder = eng
 
     def decode(self, zs):

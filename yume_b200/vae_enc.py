@@ -213,7 +213,7 @@ class Wan22VaeEncoder(WanVaeEncoder):
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 160, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
         dims = [dim * u for u in [1] + list(dim_mult)]                               # vae2_2.py:527
         layers = [Layer("in", "encoder.conv1", 64, dims[0], 4, 2)]
         for i in range(len(dim_mult)):                             # Down_ResidualBlock (:420-459)
@@ -225,7 +225,7 @@ class Wan22VaeEncoder(WanVaeEncoder):
             if down:
                 layers.append(Layer("down", f"{p}.{num_res_blocks}", co, co, ft, 2))
             layers.append(Layer("avgdown", ci=ci, co=co, ft=ft, fs=2 if down else 1))
-        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device)
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
         if self._one_pass:
@@ -241,7 +241,7 @@ class Wan21VaeEncoder(WanVaeEncoder):
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
         dims = [dim * u for u in [1] + list(dim_mult)]
         layers, n = [Layer("in", "encoder.conv1", 64, dims[0], 4, 1)], 0
         for i in range(len(dim_mult)):
@@ -252,7 +252,7 @@ class Wan21VaeEncoder(WanVaeEncoder):
             if i != len(dim_mult) - 1:
                 layers.append(Layer("down", f"encoder.downsamples.{n}", co, co, 2 if temperal_downsample[i] else 1, 2))
                 n += 1
-        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device)
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
         if self._one_pass:
@@ -261,16 +261,17 @@ class Wan21VaeEncoder(WanVaeEncoder):
             ops.nchw_to_nhwc_bf16_win(v, dst)
 
 
-def install_wan22_vae_encoder(vae, device="cuda"):
+def install_wan22_vae_encoder(vae, device="cuda", precision: str = "bf16"):
     """Attach a Wan22VaeEncoder to a live reference `Wan2_2_VAE` wrapper and re-bind its `encode(videos)` (list in / list out,
-    a non-list logs the TypeError and returns None: vae2_2.py:1045-1057)."""
+    a non-list logs the TypeError and returns None: vae2_2.py:1045-1057). precision: "bf16" only (encodes stay bf16)."""
     m = vae.model
     sd = dict(m.state_dict())
     mean, inv_std = vae.scale
     dim_mult = list(m.dim_mult)
     eng = Wan22VaeEncoder(sd, dim=sd["encoder.conv1.weight"].shape[0], z_dim=m.z_dim, dim_mult=dim_mult,
                           num_res_blocks=m.num_res_blocks, temperal_downsample=list(m.temperal_downsample),
-                          mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device)
+                          mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device,
+                          precision=precision)
     vae._yb_encoder = eng
 
     def encode(self, videos, cache=True):
@@ -284,12 +285,13 @@ def install_wan22_vae_encoder(vae, device="cuda"):
     return vae
 
 
-def install_wan21_vae_encoder(vae, device="cuda"):
-    """Attach a Wan21VaeEncoder to a live reference `WanVAE` wrapper and re-bind its `encode(videos)` (vae.py:645-653)."""
+def install_wan21_vae_encoder(vae, device="cuda", precision: str = "bf16"):
+    """Attach a Wan21VaeEncoder to a live reference `WanVAE` wrapper and re-bind its `encode(videos)` (vae.py:645-653).
+    precision: "bf16" only (encodes stay bf16)."""
     m = vae.model
     eng = Wan21VaeEncoder(dict(m.state_dict()), dim=m.dim, z_dim=m.z_dim, dim_mult=list(m.dim_mult),
                           num_res_blocks=m.num_res_blocks, temperal_downsample=list(m.temperal_downsample),
-                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device)
+                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device, precision=precision)
     vae._yb_encoder = eng
 
     def encode(self, videos):

@@ -12,7 +12,7 @@ import torch
 from ._lib import YumeB200Error
 
 Tensor = torch.Tensor
-_BF16, _F32 = torch.bfloat16, torch.float32
+_BF16, _F32, _E4M3 = torch.bfloat16, torch.float32, torch.float8_e4m3fn
 
 
 def _rup(v: int, m: int) -> int:
@@ -38,9 +38,17 @@ class WanVaeEngine:
     _chunk, _more, _carry = 0, False, None
     HIST = 2                     # carried frames of a 3-tap causal conv (the reference's CACHE_T)
     MEM_MARGIN = 2 << 30         # bytes of free device memory the chunk planner leaves unused
+    PRECISIONS = ("bf16",)       # precision= values the engine accepts (Wan22VaeDecoder adds "fp8")
+    # precision="fp8": the convs that run on e4m3 operands (Wan22VaeDecoder._repack decides), name -> (Wq e4m3 [cop, taps*cp],
+    # s_w f32 [cop], bias f32 [cop], taps). Their input streams are (e4m3 frames, scale frames) pairs, see _hist_buf.
+    conv8: Dict[str, Tuple[Tensor, Tensor, Tensor, tuple]] = {}
 
     def __init__(self, sd: Dict[str, Tensor], z_dim: int, layers: List[Layer], mean: Optional[Tensor], std: Optional[Tensor],
-                 device):
+                 device, precision: str = "bf16"):
+        if precision not in self.PRECISIONS:
+            raise YumeB200Error(f"{type(self).__name__} supports precision {' or '.join(map(repr, self.PRECISIONS))}, got "
+                                f"{precision!r} (the fp8 path is Wan22VaeDecoder's decode only)")
+        self.precision = precision
         self.device = torch.device(device)
         self.z_dim, self.layers = z_dim, layers
         mean = torch.zeros(z_dim) if mean is None else mean
@@ -113,40 +121,56 @@ class WanVaeEngine:
         """The running chunk is the whole sequence: it issues the one-pass launches."""
         return self._chunk == 0 and not self._more
 
-    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0) -> Tensor:
+    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0, fp8: bool = False):
         """Input buffer [h + T, H, W, Cp] of a conv whose input stream is `key`: after the first chunk its first h frames (n, or
-        HIST when n is 0) are the frames carried from the previous chunk and the producer writes the T new frames behind them."""
+        HIST when n is 0) are the frames carried from the previous chunk and the producer writes the T new frames behind them.
+        fp8: the pair (e4m3 [h + T, H, W, Cp], f32 scales [h + T, Cp / 128, H, W]) of an e4m3 conv's input, frames carried alike."""
         h = (n or self.HIST) if (key is not None and self._chunk > 0) else 0
+        if fp8:
+            buf = (self._new(h + T, H, W, Cp, dtype=_E4M3), self._new(h + T, Cp // 128, H, W, dtype=_F32))
+            if h:
+                for b, c in zip(buf, self._carry[key]):
+                    b[:h].copy_(c)
+            return buf
         buf = torch.zeros(h + T, H, W, Cp, device=self.device, dtype=_BF16) if zero else self._new(h + T, H, W, Cp)
         if h:
             buf[:h].copy_(self._carry[key])
         return buf
 
-    def _keep(self, key: str, frames: Tensor, n: int = 0) -> None:
+    def _keep(self, key: str, frames, n: int = 0) -> None:
         """Carry the last n (0: HIST) frames of the input stream `key` into the next chunk (zero frames in front where the stream
-        is shorter: the causal zero padding)."""
+        is shorter: the causal zero padding; for an e4m3 stream, zero values with zero scales)."""
         if not self._more:
             return
         n = n or self.HIST
-        if frames.shape[0] >= n:
-            self._carry[key] = frames[frames.shape[0] - n:].clone()
-        else:
-            c = torch.zeros(n, *frames.shape[1:], device=self.device, dtype=_BF16)
-            c[n - frames.shape[0]:].copy_(frames)
-            self._carry[key] = c
 
-    def _conv(self, name: str, a: Tensor, dims, epilogue=None, res: Optional[Tensor] = None, out: Optional[Tensor] = None,
+        def last(f: Tensor) -> Tensor:
+            if f.shape[0] >= n:
+                return f[f.shape[0] - n:].clone()
+            c = torch.zeros(n, *f.shape[1:], device=self.device, dtype=f.dtype)
+            c[n - f.shape[0]:].copy_(f)
+            return c
+        self._carry[key] = tuple(last(f) for f in frames) if isinstance(frames, tuple) else last(frames)
+
+    def _conv(self, name: str, a, dims, epilogue=None, res: Optional[Tensor] = None, out: Optional[Tensor] = None,
               out_t_mul: int = 1, out_t_add: int = 0, stride_t: int = 1, stride_hw: int = 1, key: Optional[str] = None) -> Tensor:
         """a bf16 [h + T, H, W, Cp] (unpadded, dense; h carried frames in front, see _hist_buf) -> [To*Ho*Wo (or interleaved
-        frames), cop]. `key`: the input stream whose last frames the next chunk needs."""
+        frames), cop]. `key`: the input stream whose last frames the next chunk needs. An e4m3 conv (conv8) takes the pair
+        _hist_buf(fp8=True) made and writes bf16 rows."""
         ops = self.ops
-        w, b, taps = self.conv[name]
         T, H, W = dims
-        h = a.shape[0] - T
         if key is not None:                                      # a stride-2 time_conv carries one frame (vae2_2.py:158-170)
             self._keep(key, a, 1 if stride_t > 1 else self.HIST)
         if epilogue is None:
             epilogue = ops.YB_EPI_RES_BF16 if res is not None else ops.YB_EPI_BF16
+        if isinstance(a, tuple):
+            w8, sw, b, taps = self.conv8[name]
+            if out is None:
+                out = self._new(T * H * W, w8.shape[0])
+            ops.conv3d_fp8(a[0], a[1], w8, sw, b, out, T, H, W, a[0].shape[0] - T, epilogue, res, taps=taps)
+            return out
+        w, b, taps = self.conv[name]
+        h = a.shape[0] - T
         if out is None:
             To, Ho, Wo = ops.conv_out_dims(T, H, W, taps, stride_t, stride_hw)
             out = self._new(To * Ho * Wo, w.shape[0], dtype=_F32 if epilogue == ops.YB_EPI_F32 else _BF16)
@@ -159,24 +183,31 @@ class WanVaeEngine:
         return out
 
     def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1, key: Optional[str] = None,
-             n: int = 0) -> Tensor:
+             n: int = 0, conv: Optional[str] = None):
+        """The input buffer of the conv `conv` (see _hist_buf): RMS_norm * gamma, SiLU, 2x upsample of x; an e4m3 pair when that
+        conv is one of conv8."""
         ops = self.ops
         T, H, W = dims
+        g = self.gamma[gamma] if gamma else None
+        if conv in self.conv8:
+            q, s = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n, fp8=True)
+            ops.vae_rms_act_fp8(x, dims, q[q.shape[0] - T:], s[s.shape[0] - T:], g, up, silu)
+            return q, s
         out = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n)
-        ops.vae_rms_act(x, dims, out[out.shape[0] - T:], self.gamma[gamma] if gamma else None, up, silu)
+        ops.vae_rms_act(x, dims, out[out.shape[0] - T:], g, up, silu)
         return out
 
     def _res_block(self, p: str, x: Tensor, dims) -> Tensor:
         """ResidualBlock (vae2_2.py:195-239)."""
         ops = self.ops
         c1, c2 = p + ".residual.2", p + ".residual.6"
-        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1), dims, key=c1)
+        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1, conv=c1), dims, key=c1)
         res = x
         if (p + ".shortcut") in self.lin:
             w, b = self.lin[p + ".shortcut"]
             res = self._new(x.shape[0], w.shape[0])
             ops.gemm(x, w, b, res, ops.YB_EPI_BF16)
-        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2), dims, res=res, key=c2)
+        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2, conv=c2), dims, res=res, key=c2)
 
     def _attention(self, p: str, x: Tensor, dims) -> Tensor:
         """AttentionBlock (vae2_2.py:242-283): per-frame single-head attention over H*W tokens, d = C."""
