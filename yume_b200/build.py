@@ -16,7 +16,7 @@ ROOT = Path(__file__).resolve().parent
 CSRC = ROOT / "csrc"
 LIB = CSRC / "libyume_b200.so"
 SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "vae_elementwise.cu", "probe.cu", "clip.cu", "t5.cu", "gemm_fp8.cu",
-           "attention_fp8.cu", "conv_fp8.cu"]
+           "attention_fp8.cu"]
 HEADERS = ["yb_ptx.cuh", "yb_host.h", "../../include/yume_b200.h", "../../include/yume_b200_clip.h",
            "../../include/yume_b200_t5.h", "../../include/yume_b200_stream.h",
            "../../include/yume_b200_fp8.h", "../../include/yume_b200_fp8_attn.h",

@@ -80,24 +80,6 @@ struct AttCfg {
   static_assert(SMEM_BYTES <= 227 * 1024, "shared memory budget");
 };
 
-// mbar_wait for the consumer warpgroups: the same bounded wait, but the trap is an asm statement followed by a break
-// instead of the noreturn __trap(). A noreturn call inside the setmaxnreg.inc region makes ptxas allocate the region within
-// the launch's 168 registers rather than 232, and the pipelined loop below then spills.
-__device__ __forceinline__ void att_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > YB_WAIT_LIMIT_CYCLES) {
-#ifdef YB_DEBUG_WAIT
-      printf("yb: attention consumer mbarrier wait timeout block=(%d,%d) thread=%d bar=%u parity=%u\n", blockIdx.x,
-             blockIdx.y, threadIdx.x, smem_u32(bar), parity);
-#endif
-      asm volatile("trap;");
-      break;
-    }
-  }
-}
-
 template <bool P_SMEM>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,

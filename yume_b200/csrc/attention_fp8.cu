@@ -58,16 +58,6 @@ struct Att8Params {
   float* ws_ml;           // [tail CTAs, 256, 2]   (row max in the log2 domain, row sum of p)
 };
 
-// D (64 x 128, fp32) (+)= A (64 x 32 e4m3, smem K-major) * B (128 x 32 e4m3, smem K-major)
-__device__ __forceinline__ void wgmma_ss_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %66, 0;\n\t"
-      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-      : "l"(adesc), "l"(bdesc), "r"(accumulate));
-}
-
 // D (64 x 128, fp32) (+)= A (64 x 32 e4m3, registers) * B (128 x 32 e4m3, smem K-major). A fragment of the thread (lane l of
 // warp w, t = l % 4): a[0] row 16w + l/4, k 4t .. 4t+3 (byte 0 first); a[1] the row 8 further down; a[2], a[3] the same at
 // k 16 + 4t .. 16 + 4t + 3.
@@ -80,31 +70,12 @@ __device__ __forceinline__ void wgmma_rs_e4m3(float (&d)[64], const uint32_t (&a
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));
 }
 
-// two floats -> two e4m3 bytes (lo = first), round to nearest even, saturating to +-448, NaN kept
-__device__ __forceinline__ uint32_t a8_cvt_e4m3x2(float lo, float hi) {
-  uint16_t r;
-  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
-  return r;
-}
-
 // tile row of the thread's fragment row a (row b = + 8) for the consumer warpgroups, re-derived from %tid.x at each use: a
 // value held across the KV loop is what ptxas spills first in this kernel
 __device__ __forceinline__ int a8_row_a() {
   uint32_t t;
   asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
   return static_cast<int>((t >> 7) - 1) * 64 + static_cast<int>((t >> 5) & 3) * 16 + static_cast<int>((t & 31) >> 2);
-}
-
-// the consumers' bounded wait (see att_wait in attention.cu: no noreturn call inside the setmaxnreg.inc region)
-__device__ __forceinline__ void a8_wait(uint64_t* bar, uint32_t parity) {
-  if (mbar_try_wait(bar, parity)) return;
-  const long long t0 = clock64();
-  while (!mbar_try_wait(bar, parity)) {
-    if (clock64() - t0 > YB_WAIT_LIMIT_CYCLES) {
-      asm volatile("trap;");
-      break;
-    }
-  }
 }
 
 __global__ void __launch_bounds__(A8_THREADS, 1)
@@ -185,7 +156,7 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     const uint32_t sQ = smem_u32(smem + A8_Q_OFF) + wg * 64 * 128;
     auto issue_s = [&](float (&s)[64], int itk) {
       const int slot_k = itk % NS;
-      a8_wait(&kv_full[slot_k], (itk / NS) & 1);
+      att_wait(&kv_full[slot_k], (itk / NS) & 1);
       const uint32_t sK = smem_u32(smem + A8_KV_OFF + slot_k * A8_TILE_BYTES);
       const uint64_t qd = make_smem_desc_sw128(sQ, 16, 1024), kd = make_smem_desc_sw128(sK, 16, 1024);
       wgmma_fence();
@@ -195,7 +166,7 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
     };
     int it = 0;
     for (int X = 0; X < nx; ++X) {
-      a8_wait(q_full, X);
+      att_wait(q_full, X);
       float o[64];
 #pragma unroll
       for (int i = 0; i < 64; ++i) o[i] = 0.f;
@@ -263,10 +234,10 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
 #pragma unroll
         for (int kk = 0; kk < 4; ++kk) {
           const float* e = s + 16 * kk;
-          pa[kk][0] = a8_cvt_e4m3x2(e[0], e[1]) | (a8_cvt_e4m3x2(e[4], e[5]) << 16);      // row a
-          pa[kk][1] = a8_cvt_e4m3x2(e[2], e[3]) | (a8_cvt_e4m3x2(e[6], e[7]) << 16);      // row b
-          pa[kk][2] = a8_cvt_e4m3x2(e[8], e[9]) | (a8_cvt_e4m3x2(e[12], e[13]) << 16);    // row a, +16
-          pa[kk][3] = a8_cvt_e4m3x2(e[10], e[11]) | (a8_cvt_e4m3x2(e[14], e[15]) << 16);  // row b, +16
+          pa[kk][0] = cvt_e4m3x4(e[0], e[1], e[4], e[5]);       // row a
+          pa[kk][1] = cvt_e4m3x4(e[2], e[3], e[6], e[7]);       // row b
+          pa[kk][2] = cvt_e4m3x4(e[8], e[9], e[12], e[13]);     // row a, +16
+          pa[kk][3] = cvt_e4m3x4(e[10], e[11], e[14], e[15]);   // row b, +16
         }
       };
 
@@ -284,7 +255,7 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       auto kv_step = [&](int j, const bool next) {
         const int slot_v = (it + 1) % NS, slot_kn = (it + 2) % NS;
         if (next) issue_s(s, it + 2);
-        a8_wait(&kv_full[slot_v], ((it + 1) / NS) & 1);
+        att_wait(&kv_full[slot_v], ((it + 1) / NS) & 1);
         const uint64_t vd = make_smem_desc_sw128(smem_u32(smem + A8_KV_OFF + slot_v * A8_TILE_BYTES), 16, 1024);
         wgmma_fence();
 #pragma unroll
@@ -401,8 +372,8 @@ quant_vt_fp8_kernel(const __nv_bfloat16* __restrict__ v, long long ldv, uint8_t*
   amax = wmax[0];
 #pragma unroll
   for (int w = 1; w < 8; ++w) amax = fmaxf(amax, wmax[w]);
-  float inv = __fdiv_rn(448.0f, amax), sc = __fdiv_rn(amax, 448.0f);
-  if (!(inv <= 3.402823466e38f)) { inv = 0.f; sc = 0.f; }
+  float inv, sc;
+  group_scale(amax, inv, sc);
   if (tid == 0) v_scale[static_cast<long long>(head) * (Lkp / 128) + j] = sc;
   const int d = tid & 127, f0 = (tid >> 7) * 64;
   uint8_t* orow = vt8 + (static_cast<long long>(head) * 128 + d) * Lkp + j * 128 + f0;
@@ -418,40 +389,10 @@ quant_vt_fp8_kernel(const __nv_bfloat16* __restrict__ v, long long ldv, uint8_t*
         const int key = 32 * (f >> 5) + vt_pi(f & 31);
         x[e] = __bfloat162float(tile[key * VT_PITCH + d]) * inv;
       }
-      w[q] = a8_cvt_e4m3x2(x[0], x[1]) | (a8_cvt_e4m3x2(x[2], x[3]) << 16);
+      w[q] = cvt_e4m3x4(x[0], x[1], x[2], x[3]);
     }
     *reinterpret_cast<uint4*>(orow + 16 * c) = make_uint4(w[0], w[1], w[2], w[3]);
   }
-}
-
-// 2-D tensor maps: e4m3 [rows, cols] with row stride ld bytes, box 128 x 128, 128B swizzle; f32 scales [groups, ld] read as
-// [groups][n] with box {128, 1} (entries past n are zero fill)
-static int a8_tmap_e4m3(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (!fn) return YB_ERR_NO_DRIVER;
-  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || (ld & 0xF)) return YB_ERR_ALIGNMENT;
-  cuuint64_t gdim[2] = {cols, rows};
-  cuuint64_t gstride[1] = {ld};
-  cuuint32_t box[2] = {128, 128};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
-}
-
-static int a8_tmap_scales(CUtensorMap* tm, const void* base, uint64_t n, uint64_t groups, uint64_t ld) {
-  PFN_encodeTiled fn = get_encode_fn();
-  if (!fn) return YB_ERR_NO_DRIVER;
-  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || (ld % 4)) return YB_ERR_ALIGNMENT;
-  cuuint64_t gdim[2] = {n, groups};
-  cuuint64_t gstride[1] = {ld * 4};
-  cuuint32_t box[2] = {128, 1};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
 }
 
 }  // namespace yb
@@ -481,15 +422,15 @@ extern "C" int yb_attention_fp8(const void* q8, long long ldq, const void* k8, l
   const int nkv = (Lk + 127) / 128;
   const uint64_t cols = static_cast<uint64_t>(heads) * 128;
   CUtensorMap tmQ, tmK, tmV, tmSQ, tmSK;
-  int rc = a8_tmap_e4m3(&tmQ, q8, Lq, cols, ldq);
+  int rc = make_tmap_e4m3_2d(&tmQ, q8, Lq, cols, ldq);
   if (rc) return rc;
-  rc = a8_tmap_e4m3(&tmK, k8, Lk, cols, ldk);
+  rc = make_tmap_e4m3_2d(&tmK, k8, Lk, cols, ldk);
   if (rc) return rc;
-  rc = a8_tmap_e4m3(&tmV, vt8, cols, static_cast<uint64_t>(nkv) * 128, static_cast<uint64_t>(nkv) * 128);
+  rc = make_tmap_e4m3_2d(&tmV, vt8, cols, static_cast<uint64_t>(nkv) * 128, static_cast<uint64_t>(nkv) * 128);
   if (rc) return rc;
-  rc = a8_tmap_scales(&tmSQ, qk_scale, Lq, 2 * static_cast<uint64_t>(heads), lds);
+  rc = make_tmap_f32_scales(&tmSQ, qk_scale, Lq, 2 * static_cast<uint64_t>(heads), lds);
   if (rc) return rc;
-  rc = a8_tmap_scales(&tmSK, qk_scale, Lk, 2 * static_cast<uint64_t>(heads), lds);
+  rc = make_tmap_f32_scales(&tmSK, qk_scale, Lk, 2 * static_cast<uint64_t>(heads), lds);
   if (rc) return rc;
 
   Att8Params p;

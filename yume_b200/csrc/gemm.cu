@@ -35,7 +35,6 @@ namespace yb {
 constexpr int GEMM_BLOCK_M = 128;
 constexpr int GEMM_BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
 constexpr int GEMM_THREADS = 384;
-constexpr int GEMM_GROUP_N = 8;   // rasterisation: n-tiles per group (keeps A and B footprints L2 resident)
 constexpr int GEMM_MAX_STAGES = 8;
 constexpr int GEMM_SMEM_BYTES = 227 * 1024;                 // the H100 per-block maximum
 constexpr int GEMM_A_BYTES = GEMM_BLOCK_M * GEMM_BLOCK_K * 2;
@@ -114,16 +113,6 @@ __host__ __device__ constexpr int gemm_epi_bytes(bool tma) { return tma ? GEMM_E
 static int gemm_stages(int block_n, int convw, int epi_bytes) {
   const int s = (GEMM_SMEM_BYTES - 1024 - 256 - epi_bytes - gemm_a_ring_bytes(convw)) / gemm_stage_bytes(block_n, convw);
   return s > GEMM_MAX_STAGES ? GEMM_MAX_STAGES : s;
-}
-
-__device__ __forceinline__ void tile_coords(int tile, int num_m_tiles, int num_n_tiles, int& m_tile, int& n_tile) {
-  const int per_group = GEMM_GROUP_N * num_m_tiles;
-  const int g = tile / per_group;
-  const int r = tile - g * per_group;
-  const int n_first = g * GEMM_GROUP_N;
-  const int n_in_group = min(GEMM_GROUP_N, num_n_tiles - n_first);
-  m_tile = r / n_in_group;
-  n_tile = n_first + (r - m_tile * n_in_group);
 }
 
 // One 32-column chunk of the 16 tile rows of a consumer warp, already transposed into `stage` (row pitch 36 floats) by the

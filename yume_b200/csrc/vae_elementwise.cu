@@ -7,6 +7,7 @@
 //   layout converters and the tile cross-fade (autoencoder_kl_causal_3d.py:343-359)
 #include "yb_host.h"
 #include "../../include/yume_b200_stream.h"
+#include "../../include/yume_b200_fp8_vae.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -403,6 +404,119 @@ rms_act_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16
   }
 }
 
+// ------------------------------------------------------------------------------------------------
+// RMS_norm (* gamma) -> SiLU -> nearest 2x upsample -> bf16 rounding -> 1x128 e4m3 quantisation per voxel.
+// Lane layout and fp32 arithmetic are those of rms_act_kernel<NCH, G> above for the same C / Cp, so the bf16 values
+// are the ones yb_vae_rms_act stores. Chunk c (8 channels) of a voxel sits on lane gl = c % G, so the 16 chunks of one 128-channel
+// group are 16 adjacent lanes (G is 16 or 32 here): the group max is a 4-step shuffle over them.
+// ------------------------------------------------------------------------------------------------
+template <int NCH, int G>
+__global__ void __launch_bounds__(256, 2)
+rms_act_fp8_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, uint8_t* __restrict__ out, float* __restrict__ out_scale,
+                   const float* __restrict__ gamma, int T, int Hs, int Ws, int C, int Cp, int f, int silu) {
+  static_assert(G == 16 || G == 32, "a 128-channel group spans 16 lanes");
+  constexpr int U = 4 / NCH;
+  constexpr int SUB = 32 / G;
+  constexpr int VPI = U * SUB;
+  const int H = Hs * f, W = Ws * f;
+  const int HW = H * W;
+  const int nvox = T * HW;
+  const int lane = threadIdx.x & 31;
+  const int gl = lane % G, sub = lane / G;
+  const int cch = C >> 3, pch = Cp >> 3;
+  const int groups = Cp >> 7;
+  const float sqrt_c = sqrtf(static_cast<float>(C));
+  const int stride = gridDim.x * 8 * VPI;
+  for (int v0 = (blockIdx.x * 8 + (threadIdx.x >> 5)) * VPI; v0 < nvox; v0 += stride) {
+    uint4 raw[U][NCH];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int v = v0 + u * SUB + sub;
+      int src = v;
+      if (f != 1) {
+        const int w = v % W, r = v / W;
+        const int h = r % H, t = r / H;
+        src = (t * Hs + h / f) * Ws + w / f;
+      }
+      const __nv_bfloat16* xs = x + static_cast<long long>(src) * ldx;
+#pragma unroll
+      for (int j = 0; j < NCH; ++j) {
+        const int c = gl + G * j;
+        raw[u][j] = (v < nvox && c < cch) ? *reinterpret_cast<const uint4*>(xs + c * 8) : make_uint4(0u, 0u, 0u, 0u);
+      }
+    }
+    float scl[U];
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      float ss = 0.f;
+#pragma unroll
+      for (int j = 0; j < NCH; ++j) {
+        const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw[u][j]);
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 a = __bfloat1622float2(hh[k]);
+          ss += a.x * a.x + a.y * a.y;
+        }
+      }
+      scl[u] = ss;
+    }
+    if (gamma) {
+#pragma unroll
+      for (int o = G / 2; o > 0; o >>= 1) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) scl[u] += __shfl_xor_sync(0xffffffffu, scl[u], o);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < U; ++u) {
+      const int v = v0 + u * SUB + sub;   // every lane takes part in the shuffles below; only the stores check v
+      const float sc = gamma ? sqrt_c / fmaxf(sqrtf(scl[u]), 1e-12f) : 1.f;
+#pragma unroll
+      for (int j = 0; j < NCH; ++j) {
+        const int c = gl + G * j;
+        float y[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+        if (c < cch) {
+          const __nv_bfloat162* hh = reinterpret_cast<const __nv_bfloat162*>(&raw[u][j]);
+#pragma unroll
+          for (int k = 0; k < 4; ++k) {
+            const float2 a = __bfloat1622float2(hh[k]);
+            y[2 * k] = a.x;
+            y[2 * k + 1] = a.y;
+          }
+          if (gamma) {
+            const float4 g0 = __ldg(reinterpret_cast<const float4*>(gamma + c * 8));
+            const float4 g1 = __ldg(reinterpret_cast<const float4*>(gamma + c * 8 + 4));
+            const float gg[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
+#pragma unroll
+            for (int k = 0; k < 8; ++k) y[k] = y[k] * sc * gg[k];
+          }
+          if (silu) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) y[k] = y[k] / (1.f + __expf(-y[k]));
+          }
+#pragma unroll
+          for (int k = 0; k < 8; ++k) y[k] = __bfloat162float(__float2bfloat16_rn(y[k]));   // the value yb_vae_rms_act stores
+        }
+        float amax = 0.f;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) amax = fmaxf(amax, fabsf(y[k]));
+#pragma unroll
+        for (int o = 8; o > 0; o >>= 1) amax = fmaxf(amax, __shfl_xor_sync(0xffffffffu, amax, o));
+        if (v >= nvox || c >= pch) continue;
+        float inv, scale;
+        group_scale(amax, inv, scale);
+        *reinterpret_cast<uint2*>(out + static_cast<long long>(v) * Cp + c * 8) =
+            make_uint2(cvt_e4m3x4(y[0] * inv, y[1] * inv, y[2] * inv, y[3] * inv),
+                       cvt_e4m3x4(y[4] * inv, y[5] * inv, y[6] * inv, y[7] * inv));
+        if ((c & 15) == 0) {
+          const int t = v / HW;
+          out_scale[(static_cast<long long>(t) * groups + (c >> 4)) * HW + (v - t * HW)] = scale;
+        }
+      }
+    }
+  }
+}
+
 // main[f', h', w', oc] += x[t, h, w, ci]: the DupUp3D shortcut (:376-418) of Up_ResidualBlock (:499-503) on the whole
 // sequence, first `drop` duplicated frames dropped (ft-1 on the first chunk of a sequence, 0 on the chunks after it).
 // d = f' + drop, t = d / ft, a = d % ft, e = ((oc*ft + a)*fs + b)*fs + c, ci = e / rep with rep = out_c*ft*fs*fs / in_c.
@@ -669,6 +783,35 @@ extern "C" int yb_vae_rms_act(const void* x, long long ldx, void* out, const voi
   else YB_RMS_LAUNCH(1, 8);
 #undef YB_RMS_LAUNCH
   return check_launch("vae_rms_act");
+}
+
+extern "C" int yb_vae_rms_act_fp8(const void* x, long long ldx, void* out, void* out_scale, const void* gamma, int T, int Hs, int Ws,
+                                  int C, int Cp, int up, int silu, void* stream_) {
+  if (!x || !out || !out_scale || T <= 0 || Hs <= 0 || Ws <= 0 || C <= 0) return YB_ERR_ARG;
+  if (C % 8 != 0 || C > 1024 || Cp % 128 != 0 || Cp != (C + 127) / 128 * 128 || (up != 1 && up != 2)) return YB_ERR_SHAPE;
+  if ((ldx % 8) || (reinterpret_cast<uintptr_t>(x) & 0xF) || (reinterpret_cast<uintptr_t>(out) & 0xF) ||
+      (reinterpret_cast<uintptr_t>(out_scale) & 0x3))
+    return YB_ERR_ALIGNMENT;
+  if (gamma && (reinterpret_cast<uintptr_t>(gamma) & 0xF)) return YB_ERR_ALIGNMENT;
+  const long long nvox = static_cast<long long>(T) * Hs * up * Ws * up;
+  if (nvox > 0x7fffffffLL - (1LL << 24)) return YB_ERR_SHAPE;
+  // the (NCH, G) instance yb_vae_rms_act takes for this C / Cp (Cp >= 128 here, so G is 16 or 32)
+  const int nch = C <= 256 ? 1 : (C <= 512 ? 2 : 4);
+  const int g = nch > 1 ? 32 : (Cp <= 128 ? 16 : 32);
+  const int per_block = 8 * (4 / nch) * (32 / g);
+  long long blocks = (nvox + per_block - 1) / per_block;
+  if (blocks > static_cast<long long>(sm_count()) * 32) blocks = static_cast<long long>(sm_count()) * 32;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+#define YB_RMS8_LAUNCH(NCH, G)                                                                                          \
+  rms_act_fp8_kernel<NCH, G><<<static_cast<int>(blocks), 256, 0, st>>>(                                                 \
+      static_cast<const __nv_bfloat16*>(x), ldx, static_cast<uint8_t*>(out), static_cast<float*>(out_scale),            \
+      static_cast<const float*>(gamma), T, Hs, Ws, C, Cp, up, silu)
+  if (nch == 4) YB_RMS8_LAUNCH(4, 32);
+  else if (nch == 2) YB_RMS8_LAUNCH(2, 32);
+  else if (g == 32) YB_RMS8_LAUNCH(1, 32);
+  else YB_RMS8_LAUNCH(1, 16);
+#undef YB_RMS8_LAUNCH
+  return check_launch("vae_rms_act_fp8");
 }
 
 static int dupup_launch(void* main_, const void* x, int Ts, int Hs, int Ws, int in_c, int out_c, int ft, int fs, bool first,

@@ -45,6 +45,38 @@ inline int make_tmap_bf16_2d(CUtensorMap* tm, const void* base, uint64_t rows, u
   return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
 }
 
+// 2D e4m3 tensor map: global view [rows, cols] with row stride `ld` bytes, box 128 x 128 (one 128-byte swizzle row of 128
+// e4m3 is one scale group), 128-byte swizzle, out-of-bounds elements are filled with zeros.
+inline int make_tmap_e4m3_2d(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t cols, uint64_t ld) {
+  PFN_encodeTiled fn = get_encode_fn();
+  if (!fn) return YB_ERR_NO_DRIVER;
+  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || (ld & 0xF)) return YB_ERR_ALIGNMENT;
+  cuuint64_t gdim[2] = {cols, rows};
+  cuuint64_t gstride[1] = {ld};
+  cuuint32_t box[2] = {128, 128};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
+}
+
+// f32 scale table of the e4m3 operands, [groups, ld] read as [groups][n]: box {128 entries of one group}, no swizzle, entries
+// past n are zero fill.
+inline int make_tmap_f32_scales(CUtensorMap* tm, const void* base, uint64_t n, uint64_t groups, uint64_t ld) {
+  PFN_encodeTiled fn = get_encode_fn();
+  if (!fn) return YB_ERR_NO_DRIVER;
+  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || (ld % 4)) return YB_ERR_ALIGNMENT;
+  cuuint64_t gdim[2] = {n, groups};
+  cuuint64_t gstride[1] = {ld * 4};
+  cuuint32_t box[2] = {128, 1};
+  cuuint32_t estr[2] = {1, 1};
+  CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstride, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
+}
+
 // 2D output tensor map (bf16 or fp32, `elem_bytes` 2 / 4) for TMA stores and reduce-adds: global view [rows, cols] with row
 // stride `ld` elements, boxes of box_rows x 128 bytes, 128-byte swizzle. Writes outside [rows, cols] are dropped, so a view
 // narrower than its buffer (ld > cols) leaves the columns past `cols` untouched.

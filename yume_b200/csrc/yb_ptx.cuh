@@ -1,5 +1,6 @@
 // yb_ptx.cuh — thin inline-PTX wrappers for sm_90a (H100): mbarrier, TMA (cp.async.bulk.tensor loads with cluster multicast,
-// stores and reduce-adds), cluster barriers / remote mbarrier arrivals, wgmma (warpgroup MMA) and its shared-memory descriptors.
+// stores and reduce-adds), cluster barriers / remote mbarrier arrivals, wgmma (warpgroup MMA) and its shared-memory descriptors,
+// e4m3 conversion.
 // Everything here is hand-written for sm_90a; there is no fallback path for other architectures.
 #pragma once
 #include <cstdint>
@@ -28,6 +29,19 @@ __device__ __forceinline__ void setmaxnreg_dec() {
 // barrier over the `count` threads of one role (ids 1.. are free: __syncthreads uses 0)
 __device__ __forceinline__ void named_bar_sync(int id, int count) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+
+// Tile rasterisation of the persistent GEMMs: tile -> (m_tile, n_tile), walking all m-tiles of a group of TILE_GROUP_N n-tiles
+// before the next group (keeps the A and B footprints L2 resident)
+constexpr int TILE_GROUP_N = 8;
+__device__ __forceinline__ void tile_coords(int tile, int num_m_tiles, int num_n_tiles, int& m_tile, int& n_tile) {
+  const int per_group = TILE_GROUP_N * num_m_tiles;
+  const int g = tile / per_group;
+  const int r = tile - g * per_group;
+  const int n_first = g * TILE_GROUP_N;
+  const int n_in_group = min(TILE_GROUP_N, num_n_tiles - n_first);
+  m_tile = r / n_in_group;
+  n_tile = n_first + (r - m_tile * n_in_group);
 }
 
 // ----------------------------------------------------------------------------------------------
@@ -74,6 +88,23 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
              threadIdx.x, smem_u32(bar), parity);
 #endif
       __trap();
+    }
+  }
+}
+// mbar_wait for the consumer warpgroups of the attention kernels: the same bounded wait, but the trap is an asm statement
+// followed by a break instead of the noreturn __trap(). A noreturn call inside the setmaxnreg.inc region makes ptxas allocate
+// the region within the launch's 168 registers rather than 232, and the pipelined loops then spill.
+__device__ __forceinline__ void att_wait(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > YB_WAIT_LIMIT_CYCLES) {
+#ifdef YB_DEBUG_WAIT
+      printf("yb: attention consumer mbarrier wait timeout block=(%d,%d) thread=%d bar=%u parity=%u\n", blockIdx.x,
+             blockIdx.y, threadIdx.x, smem_u32(bar), parity);
+#endif
+      asm volatile("trap;");
+      break;
     }
   }
 }
@@ -250,6 +281,15 @@ __device__ __forceinline__ void wgmma_ss_acc64(float (&d)[64], uint64_t adesc, u
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
       : "l"(adesc), "l"(bdesc), "r"(accumulate), "n"(TB));
 }
+// D (64 x 128, fp32) (+)= A (64 x 32 e4m3, smem K-major) * B (128 x 32 e4m3, smem K-major); fragment layout as wgmma_ss_n128
+__device__ __forceinline__ void wgmma_ss_e4m3(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 
 // ----------------------------------------------------------------------------------------------
 // small numeric helpers
@@ -273,6 +313,34 @@ __device__ __forceinline__ float gelu_tanh(float x) {
   const float k0 = 0.7978845608028654f, k1 = 0.044715f;
   float u = k0 * (x + k1 * x * x * x);
   return 0.5f * x * (1.0f + fast_tanh(u));
+}
+
+// ----------------------------------------------------------------------------------------------
+// e4m3 quantisation (numerics: include/yume_b200_fp8.h)
+// ----------------------------------------------------------------------------------------------
+// two floats -> two e4m3 bytes (lo = first), round to nearest even, saturating to +-448, NaN kept
+__device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(hi), "f"(lo));
+  return r;
+}
+// four floats -> four e4m3 bytes in memory order (x0 first): cvt_e4m3x2 twice, packed in one asm statement (built from two
+// cvt_e4m3x2 calls, the RMS pass of vae_elementwise.cu schedules differently)
+__device__ __forceinline__ uint32_t cvt_e4m3x4(float x0, float x1, float x2, float x3) {
+  uint32_t r;
+  asm("{\n\t.reg .b16 lo, hi;\n\t"
+      "cvt.rn.satfinite.e4m3x2.f32 lo, %2, %1;\n\t"
+      "cvt.rn.satfinite.e4m3x2.f32 hi, %4, %3;\n\t"
+      "mov.b32 %0, {lo, hi};\n\t}\n"
+      : "=r"(r) : "f"(x0), "f"(x1), "f"(x2), "f"(x3));
+  return r;
+}
+// (inv, scale) of a group with max |x| == amax (NaN excluded): inv = 448 / amax, scale = amax / 448, both 0 when inv is not
+// finite (an all-zero group)
+__device__ __forceinline__ void group_scale(float amax, float& inv, float& scale) {
+  inv = __fdiv_rn(448.0f, amax);
+  scale = __fdiv_rn(amax, 448.0f);
+  if (!(inv <= 3.402823466e38f)) { inv = 0.f; scale = 0.f; }
 }
 
 }  // namespace yb
