@@ -168,6 +168,11 @@ FP8_VAE_SIGNATURES = {
     "yb_vae_rms_act_fp8": (_i, [_vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
 }
 
+# every symbol include/yume_b200_vae_resume.h declares (the frame comparison of a resuming Wan VAE session)
+RESUME_SIGNATURES = {
+    "yb_vae_frame_match": (_i, [_vp, _i, _vp, _i, _i, _ll, _i, _vp, _vp]),
+}
+
 _lib = None
 
 
@@ -189,7 +194,7 @@ def load():
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
-                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES}.items():
+                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES, **RESUME_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

@@ -5,9 +5,11 @@
 //                     F.pad as four separate full-tensor passes: unet_causal_3d_blocks.py:72,144-174,375-379)
 //   masked_softmax    frame-causal softmax of the mid-block attention scores (:37-45, diffusers Attention)
 //   layout converters and the tile cross-fade (autoencoder_kl_causal_3d.py:343-359)
+//   frame_match       the bitwise prefix / zero-tail scan of a resuming Wan VAE session (include/yume_b200_vae_resume.h)
 #include "yb_host.h"
 #include "../../include/yume_b200_stream.h"
 #include "../../include/yume_b200_fp8_vae.h"
+#include "../../include/yume_b200_vae_resume.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -651,6 +653,57 @@ inline int grid_for(long long total) {
   return static_cast<int>(b < cap ? (b > 0 ? b : 1) : cap);
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Frame comparison of a resuming VAE session (include/yume_b200_vae_resume.h). kept [C, t_kept, nvec] and x [C, t, nvec] in
+// V-sized words. A work item is FM_VEC_PER_THREAD * 256 words of one (channel, frame) row: its threads OR together x's bits
+// and the XOR of x with kept, the block ORs the two flags, and thread 0 lowers result[0] to the frame on a difference and
+// raises result[1] past the frame on a set bit. Only the atomics depend on the order of blocks, and min / max do not.
+// ---------------------------------------------------------------------------------------------------------
+constexpr int FM_VEC_PER_THREAD = 8;
+
+__device__ __forceinline__ unsigned long long fm_bits(uint4 v) {
+  return static_cast<unsigned long long>(v.x | v.y) | (static_cast<unsigned long long>(v.z | v.w) << 32);
+}
+__device__ __forceinline__ uint4 fm_xor(uint4 a, uint4 b) { return make_uint4(a.x ^ b.x, a.y ^ b.y, a.z ^ b.z, a.w ^ b.w); }
+template <typename V> __device__ __forceinline__ unsigned long long fm_bits(V v) { return static_cast<unsigned long long>(v); }
+template <typename V> __device__ __forceinline__ V fm_xor(V a, V b) { return static_cast<V>(a ^ b); }
+
+__global__ void frame_match_init_kernel(int* result, int n_cmp) {
+  result[0] = n_cmp;
+  result[1] = 0;
+}
+
+template <typename V>
+__global__ void __launch_bounds__(256) frame_match_kernel(const V* __restrict__ kept, int t_kept, const V* __restrict__ x, int t,
+                                                          long long rows, long long nvec, int* __restrict__ result) {
+  const long long per_item = static_cast<long long>(FM_VEC_PER_THREAD) * blockDim.x;
+  const long long items_per_row = (nvec + per_item - 1) / per_item;
+  for (long long item = blockIdx.x; item < rows * items_per_row; item += gridDim.x) {
+    const long long row = item / items_per_row;
+    const long long base = (item % items_per_row) * per_item;
+    const int f = static_cast<int>(row % t);
+    const long long c = row / t;
+    const V* xr = x + row * nvec;
+    const V* kr = f < t_kept ? kept + (c * t_kept + f) * nvec : nullptr;
+    unsigned long long nz = 0, diff = 0;
+#pragma unroll
+    for (int j = 0; j < FM_VEC_PER_THREAD; ++j) {
+      const long long i = base + static_cast<long long>(j) * blockDim.x + threadIdx.x;
+      if (i < nvec) {
+        const V a = xr[i];
+        nz |= fm_bits(a);
+        if (kr) diff |= fm_bits(fm_xor(a, kr[i]));
+      }
+    }
+    const int any_nz = __syncthreads_or(nz != 0);
+    const int any_diff = __syncthreads_or(diff != 0);
+    if (threadIdx.x == 0) {
+      if (any_diff) atomicMin(result, f);
+      if (any_nz) atomicMax(result + 1, f + 1);
+    }
+  }
+}
+
 }  // namespace yb
 
 using namespace yb;
@@ -884,4 +937,31 @@ extern "C" int yb_nhwc_to_nchw_f32_clamp_win(const void* x, long long ldx, void*
   nhwc_to_nchw_kernel<<<grid_for(N * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(x), ldx, static_cast<float*>(out), N, Cn, lo, hi, plane);
   return check_launch("nhwc_to_nchw_clamp");
+}
+
+extern "C" int yb_vae_frame_match(const void* kept, int t_kept, const void* x, int t, int C, long long frame_elems,
+                                  int elem_bytes, int* result, void* stream_) {
+  if (!x || !result || t <= 0 || t_kept < 0 || C <= 0 || frame_elems <= 0 || (t_kept > 0 && !kept)) return YB_ERR_ARG;
+  if (elem_bytes != 1 && elem_bytes != 2 && elem_bytes != 4 && elem_bytes != 8) return YB_ERR_ARG;
+  if (reinterpret_cast<uintptr_t>(result) & 0x3) return YB_ERR_ALIGNMENT;
+  const long long frame_bytes = frame_elems * elem_bytes;
+  const uintptr_t addr = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(t_kept > 0 ? kept : x) |
+                         static_cast<uintptr_t>(frame_bytes);
+  const int vec = (addr & 0xF) == 0 ? 16 : (addr & 0x7) == 0 ? 8 : (addr & 0x3) == 0 ? 4 : (addr & 0x1) == 0 ? 2 : 1;
+  const long long rows = static_cast<long long>(C) * t, nvec = frame_bytes / vec;
+  const long long items = rows * ((nvec + FM_VEC_PER_THREAD * 256 - 1) / (FM_VEC_PER_THREAD * 256));
+  const long long cap = static_cast<long long>(sm_count()) * 8;
+  const int grid = static_cast<int>(items < cap ? items : cap);
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+  frame_match_init_kernel<<<1, 1, 0, st>>>(result, t_kept < t ? t_kept : t);
+#define YB_FM_LAUNCH(V)                                                                                                  \
+  frame_match_kernel<V><<<grid, 256, 0, st>>>(static_cast<const V*>(kept), t_kept, static_cast<const V*>(x), t, rows, nvec, \
+                                              result)
+  if (vec == 16) YB_FM_LAUNCH(uint4);
+  else if (vec == 8) YB_FM_LAUNCH(unsigned long long);
+  else if (vec == 4) YB_FM_LAUNCH(unsigned int);
+  else if (vec == 2) YB_FM_LAUNCH(unsigned short);
+  else YB_FM_LAUNCH(unsigned char);
+#undef YB_FM_LAUNCH
+  return check_launch("vae_frame_match");
 }

@@ -801,6 +801,28 @@ def vae_unpatchify2_clamp(y: torch.Tensor, out: torch.Tensor, T: int, H: int, W:
     return out
 
 
+def vae_frame_match(kept: Optional[torch.Tensor], x: torch.Tensor, result: torch.Tensor) -> torch.Tensor:
+    """kept [C, Tk, ...] (or None: Tk = 0) and x [C, T, ...] dense, same dtype and frame shape -> result int32 [2] on the
+    device: (first frame < min(Tk, T) at which they differ in any bit, else min(Tk, T); start of x's trailing all-zero run).
+    No synchronisation: the caller reads result when it needs the two numbers."""
+    global _launches
+    if not x.is_cuda or not x.is_contiguous() or x.dim() < 2:
+        raise YumeB200Error("vae_frame_match: x must be a contiguous CUDA tensor [C, T, ...]")
+    _need(result, torch.int32, "result")
+    if result.numel() != 2:
+        raise YumeB200Error("vae_frame_match: result must hold 2 int32")
+    C, T = x.shape[:2]
+    if kept is not None and (not kept.is_cuda or not kept.is_contiguous() or kept.dtype != x.dtype or kept.shape[0] != C
+                             or kept.shape[2:] != x.shape[2:]):
+        raise YumeB200Error("vae_frame_match: kept must be a contiguous CUDA tensor of x's dtype, channels and frame shape")
+    t_kept = 0 if kept is None else kept.shape[1]
+    frame = math.prod(x.shape[2:])
+    check(_lib.load().yb_vae_frame_match(_ptr(kept) if t_kept else None, t_kept, x.data_ptr(), T, C, frame, x.element_size(),
+                                         result.data_ptr(), _stream()), "yb_vae_frame_match")
+    _launches += 2
+    return result
+
+
 # ------------------------------------------------------------------------------------------------------------
 # FP8 block GEMMs (include/yume_b200_fp8.h). An fp8 activation is a pair: e4m3 values [M, K] and f32 1x128 group scales
 # [K / 128, lds >= M] (group-major).

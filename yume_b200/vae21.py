@@ -83,7 +83,8 @@ class Wan21VaeDecoder(WanVaeDecoder):
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_upsample: Sequence[bool] = (True, True, False),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16",
+                 resume: bool = False, **_):
         self.plan = upsample_plan(dim, dim_mult, num_res_blocks, temperal_upsample)
         layers = decoder_front(dim * dim_mult[-1])
         for n, kind, ci, co in self.plan:                        # Resample's Conv2d halves the channels (:76-83)
@@ -91,7 +92,7 @@ class Wan21VaeDecoder(WanVaeDecoder):
             ft = 2 if kind == "upsample3d" else 1
             layers.append(Layer("res", p, ci, co) if kind == "res" else Layer("up", p, ci, co, ft, 2))
         layers.append(Layer("head", "decoder.head.2", self.plan[-1][3], _rup(3, 32)))
-        super().__init__(sd, z_dim, layers, mean, std, device, precision)
+        super().__init__(sd, z_dim, layers, mean, std, device, precision, resume)
 
     def _write(self, y: Tensor, out: Tensor, dims) -> None:
         if self._one_pass:
@@ -100,13 +101,15 @@ class Wan21VaeDecoder(WanVaeDecoder):
             ops.nhwc_to_nchw_f32_win(y, out, (-1.0, 1.0))
 
 
-def install_wan21_vae(vae, device="cuda", precision: str = "bf16"):
+def install_wan21_vae(vae, device="cuda", precision: str = "bf16", resume: bool = False):
     """Attach a Wan21VaeDecoder to a live reference `WanVAE` wrapper and re-bind its `decode(zs)` (list in / list out,
-    vae.py:655-663). precision: "bf16" only (Wan21VaeDecoder rejects "fp8")."""
+    vae.py:655-663). precision: "bf16" only (Wan21VaeDecoder rejects "fp8"). resume: keep the last decode's state so that a
+    latent extending it decodes only its new frames (WanVaeEngine._resumed)."""
     m = vae.model
     eng = Wan21VaeDecoder(dict(m.state_dict()), dim=m.dim, z_dim=m.z_dim, dim_mult=list(m.dim_mult),
                           num_res_blocks=m.num_res_blocks, temperal_upsample=list(m.temperal_upsample),
-                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device, precision=precision)
+                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device, precision=precision,
+                          resume=resume)
     vae._yb_decoder = eng
 
     def decode(self, zs):

@@ -165,9 +165,14 @@ class WanVaeDecoder(WanVaeEngine):
     @torch.no_grad()
     def decode(self, z: Tensor) -> Tensor:
         """z [z_dim, T, H, W] -> the clamped video (see the class), in the chunks `plan_chunks` sizes from the free device
-        memory."""
+        memory. With resume=True a latent that extends the last call's latent runs only its new frames (WanVaeEngine._resumed)."""
         if z.dim() != 4 or z.shape[0] != self.z_dim:
             raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
+        if self.resume:
+            T, H, W = z.shape[1:]
+            src = z.to(self.device, _F32).contiguous()
+            return self._resumed(src, src.data_ptr() != z.data_ptr(), self._out_shape(T, H, W), 1, self._t_scale(),
+                                 lambda n: self.chunk_bytes(n, T, H, W), fork=False)
         return self._decode_chunks(z, self.plan_chunks(*z.shape[1:]))
 
     def _decode_chunks(self, z: Tensor, lengths: Sequence[int]) -> Tensor:
@@ -203,7 +208,8 @@ class Wan22VaeDecoder(WanVaeDecoder):
 
     def __init__(self, sd: Dict[str, Tensor], dec_dim: int = 256, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_upsample: Sequence[bool] = (True, True, False),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16",
+                 resume: bool = False, **_):
         self.dims = dims = [dec_dim * u for u in [dim_mult[-1]] + list(dim_mult[::-1])]      # vae2_2.py:656
         layers = decoder_front(dims[0])
         for i in range(len(dim_mult)):                           # Up_ResidualBlock (:461-503)
@@ -216,7 +222,7 @@ class Wan22VaeDecoder(WanVaeDecoder):
                 ft = 2 if i < len(temperal_upsample) and temperal_upsample[i] else 1
                 layers += [Layer("up", f"{p}.{num_res_blocks + 1}", co, co, ft, 2), Layer("dupup", ci=ci, co=co, ft=ft, fs=2)]
         layers.append(Layer("head", "decoder.head.2", dims[-1], _rup(12, 32)))
-        super().__init__(sd, z_dim, layers, mean, std, device, precision)
+        super().__init__(sd, z_dim, layers, mean, std, device, precision, resume)
 
     def _repack(self, sd: Dict[str, Tensor], mean: Tensor, std: Tensor) -> None:
         super()._repack(sd, mean, std)
@@ -236,9 +242,10 @@ class Wan22VaeDecoder(WanVaeDecoder):
             ops.vae_unpatchify2_clamp_win(y, out, *dims)
 
 
-def install_wan22_vae(vae, device="cuda", precision: str = "bf16"):
+def install_wan22_vae(vae, device="cuda", precision: str = "bf16", resume: bool = False):
     """Attach a Wan22VaeDecoder to a live reference `Wan2_2_VAE` wrapper and re-bind its `decode(zs)` (same list-in /
-    list-out contract and TypeError behaviour as vae2_2.py:1059-1072). precision: see Wan22VaeDecoder."""
+    list-out contract and TypeError behaviour as vae2_2.py:1059-1072). precision: see Wan22VaeDecoder. resume: keep the last
+    decode's state so that a latent extending it decodes only its new frames (WanVaeEngine._resumed)."""
     m = vae.model
     sd = dict(m.state_dict())
     dims0 = sd["decoder.conv1.weight"].shape[0]
@@ -247,7 +254,7 @@ def install_wan22_vae(vae, device="cuda", precision: str = "bf16"):
     eng = Wan22VaeDecoder(sd, dec_dim=dims0 // dim_mult[-1], z_dim=m.z_dim, dim_mult=dim_mult,
                           num_res_blocks=m.num_res_blocks, temperal_upsample=m.temperal_upsample,
                           mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device,
-                          precision=precision)
+                          precision=precision, resume=resume)
     vae._yb_decoder = eng
 
     def decode(self, zs):

@@ -185,18 +185,25 @@ class WanVaeEncoder(WanVaeEngine):
     @torch.no_grad()
     def encode(self, video: Tensor) -> Tensor:
         """video f32 [3, T, H, W] -> mu [z_dim, 1 + (T-1)//4, H/s, W/s], in the chunks `plan_chunks` sizes from the free device
-        memory."""
-        video = self._frames(video)
-        return self._encode_chunks(video, self.plan_chunks(*video.shape[1:]))
+        memory. With resume=True a video that extends the last call's video, or its frames before the trailing all-zero
+        frames, runs only its new frames (WanVaeEngine._resumed)."""
+        v = self._frames(video)
+        if self.resume:
+            _, T, H, W = v.shape
+            return self._resumed(v, v.data_ptr() != video.data_ptr(), self._mu_shape(T, H, W), 4, 1,
+                                 lambda n: self.chunk_bytes(n, T, H, W), fork=True)
+        return self._encode_chunks(v, self.plan_chunks(*v.shape[1:]))
 
     def _encode_chunks(self, video: Tensor, lengths: Sequence[int]) -> Tensor:
         """Encode in chunks of `lengths` LATENT frames (a partition of 1 + (T-1)//4): the first chunk reads 1 + 4(n-1) video
         frames, every later one 4n (the reference's frame 0, then 4 frames per call)."""
         video = self._frames(video)
-        _, T, H, W = video.shape
+        return self._chunks(video, lengths, self._mu_shape(*video.shape[1:]), 4, 1)
+
+    def _mu_shape(self, T: int, H: int, W: int):
         if H % self.SCALE or W % self.SCALE:
             raise YumeB200Error(f"Wan VAE encode needs H, W divisible by {self.SCALE}")
-        return self._chunks(video, lengths, (self.z_dim, 1 + (T - 1) // 4, H // self.SCALE, W // self.SCALE), 4, 1)
+        return self.z_dim, 1 + (T - 1) // 4, H // self.SCALE, W // self.SCALE
 
     def _fixed_bytes(self, T: int, H: int, W: int) -> int:
         """mu, and the device copy of the video `encode` makes when it is handed one on another device or not contiguous."""
@@ -213,7 +220,8 @@ class Wan22VaeEncoder(WanVaeEncoder):
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 160, z_dim: int = 48, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16",
+                 resume: bool = False, **_):
         dims = [dim * u for u in [1] + list(dim_mult)]                               # vae2_2.py:527
         layers = [Layer("in", "encoder.conv1", 64, dims[0], 4, 2)]
         for i in range(len(dim_mult)):                             # Down_ResidualBlock (:420-459)
@@ -225,7 +233,7 @@ class Wan22VaeEncoder(WanVaeEncoder):
             if down:
                 layers.append(Layer("down", f"{p}.{num_res_blocks}", co, co, ft, 2))
             layers.append(Layer("avgdown", ci=ci, co=co, ft=ft, fs=2 if down else 1))
-        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision)
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision, resume)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
         if self._one_pass:
@@ -241,7 +249,8 @@ class Wan21VaeEncoder(WanVaeEncoder):
 
     def __init__(self, sd: Dict[str, Tensor], dim: int = 96, z_dim: int = 16, dim_mult: Sequence[int] = (1, 2, 4, 4),
                  num_res_blocks: int = 2, temperal_downsample: Sequence[bool] = (False, True, True),
-                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16", **_):
+                 mean: Optional[Tensor] = None, std: Optional[Tensor] = None, device="cuda", precision: str = "bf16",
+                 resume: bool = False, **_):
         dims = [dim * u for u in [1] + list(dim_mult)]
         layers, n = [Layer("in", "encoder.conv1", 64, dims[0], 4, 1)], 0
         for i in range(len(dim_mult)):
@@ -252,7 +261,7 @@ class Wan21VaeEncoder(WanVaeEncoder):
             if i != len(dim_mult) - 1:
                 layers.append(Layer("down", f"encoder.downsamples.{n}", co, co, 2 if temperal_downsample[i] else 1, 2))
                 n += 1
-        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision)
+        super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision, resume)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
         if self._one_pass:
@@ -261,9 +270,10 @@ class Wan21VaeEncoder(WanVaeEncoder):
             ops.nchw_to_nhwc_bf16_win(v, dst)
 
 
-def install_wan22_vae_encoder(vae, device="cuda", precision: str = "bf16"):
+def install_wan22_vae_encoder(vae, device="cuda", precision: str = "bf16", resume: bool = False):
     """Attach a Wan22VaeEncoder to a live reference `Wan2_2_VAE` wrapper and re-bind its `encode(videos)` (list in / list out,
-    a non-list logs the TypeError and returns None: vae2_2.py:1045-1057). precision: "bf16" only (encodes stay bf16)."""
+    a non-list logs the TypeError and returns None: vae2_2.py:1045-1057). precision: "bf16" only (encodes stay bf16). resume:
+    keep the last encode's state so that a video extending it encodes only its new frames (WanVaeEngine._resumed)."""
     m = vae.model
     sd = dict(m.state_dict())
     mean, inv_std = vae.scale
@@ -271,7 +281,7 @@ def install_wan22_vae_encoder(vae, device="cuda", precision: str = "bf16"):
     eng = Wan22VaeEncoder(sd, dim=sd["encoder.conv1.weight"].shape[0], z_dim=m.z_dim, dim_mult=dim_mult,
                           num_res_blocks=m.num_res_blocks, temperal_downsample=list(m.temperal_downsample),
                           mean=mean.detach().float().cpu(), std=(1.0 / inv_std.detach().float()).cpu(), device=device,
-                          precision=precision)
+                          precision=precision, resume=resume)
     vae._yb_encoder = eng
 
     def encode(self, videos, cache=True):
@@ -285,13 +295,15 @@ def install_wan22_vae_encoder(vae, device="cuda", precision: str = "bf16"):
     return vae
 
 
-def install_wan21_vae_encoder(vae, device="cuda", precision: str = "bf16"):
+def install_wan21_vae_encoder(vae, device="cuda", precision: str = "bf16", resume: bool = False):
     """Attach a Wan21VaeEncoder to a live reference `WanVAE` wrapper and re-bind its `encode(videos)` (vae.py:645-653).
-    precision: "bf16" only (encodes stay bf16)."""
+    precision: "bf16" only (encodes stay bf16). resume: keep the last encode's state so that a video extending it encodes
+    only its new frames (WanVaeEngine._resumed)."""
     m = vae.model
     eng = Wan21VaeEncoder(dict(m.state_dict()), dim=m.dim, z_dim=m.z_dim, dim_mult=list(m.dim_mult),
                           num_res_blocks=m.num_res_blocks, temperal_downsample=list(m.temperal_downsample),
-                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device, precision=precision)
+                          mean=vae.mean.detach().float(), std=vae.std.detach().float(), device=device, precision=precision,
+                          resume=resume)
     vae._yb_encoder = eng
 
     def encode(self, videos):

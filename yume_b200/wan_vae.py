@@ -30,6 +30,19 @@ class Layer(NamedTuple):
     fs: int = 1             # in: patch size; up / down / shortcut: space factor
 
 
+def _frames_of(units: int, k: int) -> int:
+    """Frames of a stream that hold its first `units` latent frames, k frames per latent frame after frame 0."""
+    return 1 + (units - 1) * k if units else 0
+
+
+class _Kept(NamedTuple):
+    """What a resuming engine keeps from its last call (WanVaeEngine._resumed)."""
+    src: Tensor                     # its own copy of the input (device, f32)
+    out: Tensor                     # the result returned (the caller's tensor; a private copy when `version` is None)
+    version: Optional[int]          # out._version when returned: an in-place edit by the caller makes the next call run in full
+    snaps: Dict[int, Tuple[int, dict]]   # input frames P -> (latent frames, the carries after them)
+
+
 class WanVaeEngine:
     """Base of the four engines. An engine builds its layer list from its config and hands it to this constructor; its side
     (decode or encode) supplies `_repack`, the `in`, `up` / `down` and `head` steps (`_input`, `_resample`, `_head`) and `ops`,
@@ -42,13 +55,17 @@ class WanVaeEngine:
     # precision="fp8": the convs that run on e4m3 operands (Wan22VaeDecoder._repack decides), name -> (Wq e4m3 [cop, taps*cp],
     # s_w f32 [cop], bias f32 [cop], taps). Their input streams are (e4m3 frames, scale frames) pairs, see _hist_buf.
     conv8: Dict[str, Tuple[Tensor, Tensor, Tensor, tuple]] = {}
+    _kept: Optional[_Kept] = None   # resume=True: the state kept from the last call
 
     def __init__(self, sd: Dict[str, Tensor], z_dim: int, layers: List[Layer], mean: Optional[Tensor], std: Optional[Tensor],
-                 device, precision: str = "bf16"):
+                 device, precision: str = "bf16", resume: bool = False):
         if precision not in self.PRECISIONS:
             raise YumeB200Error(f"{type(self).__name__} supports precision {' or '.join(map(repr, self.PRECISIONS))}, got "
                                 f"{precision!r} (the fp8 path is Wan22VaeDecoder's decode only)")
         self.precision = precision
+        # resume=True keeps the last call's input, result and carries on the device, so that a call whose input extends the
+        # last one runs only its new latent frames (_resumed); False keeps nothing between calls
+        self.resume = bool(resume)
         self.device = torch.device(device)
         self.z_dim, self.layers = z_dim, layers
         mean = torch.zeros(z_dim) if mean is None else mean
@@ -283,16 +300,85 @@ class WanVaeEngine:
         if sum(lengths) != units or min(lengths) < 1:
             raise YumeB200Error(f"chunk lengths {list(lengths)} do not partition {units} latent frames")
         out = self._new(*out_shape, dtype=_F32)
-        t_in, t_out = 0, 0
-        self._carry = {}
+        self._stream(src, out, lengths, k_in, k_out)
+        return out
+
+    def _stream(self, src: Tensor, out: Tensor, lengths: Sequence[int], k_in: int, k_out: int, u0: int = 0,
+                carry: Optional[dict] = None, keep: bool = False, snap: int = -1):
+        """Run latent frames u0 .. u0 + sum(lengths) of `src` in chunks of `lengths` into their frame windows of `out`. u0 > 0
+        continues a stream whose carries at latent frame u0 are `carry`: every chunk is then a chunk after the first. keep: the
+        last chunk carries as if another followed (a resuming engine). Returns the carries at the end (keep) and those after
+        latent frame `snap` (when a chunk ends there), each a dict the running stream no longer writes into."""
+        t_in, t_out = _frames_of(u0, k_in), _frames_of(u0, k_out)
+        self._carry = {} if carry is None else dict(carry)
+        at_snap = None
         try:
             for i, n in enumerate(lengths):
-                self._chunk, self._more = i, i < len(lengths) - 1
-                n_in, n_out = (n * k_in, n * k_out) if i else (1 + (n - 1) * k_in, 1 + (n - 1) * k_out)
+                self._chunk, self._more = i + (1 if u0 else 0), keep or i < len(lengths) - 1
+                n_in, n_out = (n * k_in, n * k_out) if self._chunk else (1 + (n - 1) * k_in, 1 + (n - 1) * k_out)
                 self._run_chunk(src[:, t_in:t_in + n_in], out[:, t_out:t_out + n_out])
-                t_in, t_out = t_in + n_in, t_out + n_out
+                t_in, t_out, u0 = t_in + n_in, t_out + n_out, u0 + n
+                if u0 == snap:
+                    at_snap = dict(self._carry)                  # _keep replaces carries, never writes into one
+            return (dict(self._carry) if keep else None), at_snap
         finally:
             self._chunk, self._more, self._carry = 0, False, None
+
+    # ---- resuming across calls -----------------------------------------------------------------------------
+    def retained_bytes(self) -> int:
+        """Device bytes a resuming engine holds between calls: its copy of the last input, the result it returned (a reference:
+        shared with the caller while the caller keeps it) and the carried conv frames of every snapshot. 0 when nothing is
+        kept (resume=False, before the first call, after reset())."""
+        k = self._kept
+        if k is None:
+            return 0
+        seen, total = set(), 0
+        tensors = [k.src, k.out] + [t for _, c in k.snaps.values() for v in c.values()
+                                    for t in (v if isinstance(v, tuple) else (v,))]
+        for t in tensors:
+            if t.data_ptr() not in seen:
+                seen.add(t.data_ptr())
+                total += t.numel() * t.element_size()
+        return total
+
+    def reset(self) -> None:
+        """Drop the state a resuming engine keeps between calls: the next call runs in full."""
+        self._kept = None
+
+    def _resumed(self, src: Tensor, owned: bool, out_shape, k_in: int, k_out: int, nbytes, fork: bool) -> Tensor:
+        """A call of a resuming engine on `src` (on the device, f32, contiguous; `owned`: not the caller's tensor). When the kept
+        input of the last call and `src` agree bit for bit on the first P frames, P a snapshot of the kept state, only the
+        latent frames after P run, as later chunks of the kept stream; the result's first frames are the kept result's.
+        Snapshots: the end of the input, and for an encoder (`fork`) also the start of its trailing all-zero frames when that
+        is a latent-frame boundary. Anything else runs in full. Either way the state of this call replaces the kept one."""
+        kept, self._kept = self._kept, None                      # dropped if this call fails
+        units = 1 + (src.shape[1] - 1) // k_in
+        comparable = (kept is not None and kept.src.shape[0] == src.shape[0] and kept.src.shape[2:] == src.shape[2:]
+                      and (kept.version is None or kept.out._version == kept.version))
+        match = torch.empty(2, dtype=torch.int32, device=self.device)
+        self.ops.vae_frame_match(kept.src if comparable else None, src, match)
+        first, zero = match.tolist()                             # the one synchronisation a resuming call adds
+        snaps = kept.snaps if comparable else {}
+        P = max((p for p in snaps if p <= first), default=0)
+        u0, carry = snaps[P] if P else (0, None)
+        fu = 1 + (zero - 1) // k_in if fork and zero > 0 and (zero - 1) % k_in == 0 and zero < src.shape[1] else -1
+        if u0 < fu:                                              # the stream passes the fork: a chunk ends there
+            lengths = self._plan(fu - u0, nbytes) + self._plan(units - fu, nbytes)
+        else:
+            lengths = self._plan(units - u0, nbytes) if units > u0 else []
+        out = self._new(*out_shape, dtype=_F32)
+        if u0:
+            n = _frames_of(u0, k_out)
+            out[:, :n].copy_(kept.out[:, :n])
+        kept = None
+        end, at_fork = self._stream(src, out, lengths, k_in, k_out, u0, carry, keep=True, snap=fu)
+        new_snaps = {src.shape[1]: (units, end)}
+        if at_fork is not None:
+            new_snaps[zero] = (fu, at_fork)
+        elif fu > 0 and zero in snaps and zero <= first:         # the fork lies in the resumed prefix: still valid
+            new_snaps[zero] = snaps[zero]
+        version = None if out.is_inference() else out._version
+        self._kept = _Kept(src if owned else src.clone(), out if version is not None else out.clone(), version, new_snaps)
         return out
 
     # ---- chunk planner -------------------------------------------------------------------------------------
