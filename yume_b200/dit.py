@@ -570,28 +570,34 @@ class WanDiT:
                  a_split=Wh, a_split_stride=Lp * Wh, shape=(Lp, C))
         T.end("gemm_o")
 
-    def _cross_kv(self, ctx: Tensor, own_storage: bool = False):
+    def _cross_kv(self, ctx: Tensor, own_storage: bool = False, block: Optional[int] = None):
         """K | V of the embedded context for every block in one GEMM (+ the image branch for 14B), RMSNorm on the K
         halves. Returns per-block (kv_text, kv_img or None) views of [S, 2C]. own_storage: allocate fresh result buffers
-        (context-cache entries outlive the call) instead of the shared workspace."""
+        (context-cache entries outlive the call) instead of the shared workspace. block: block `block`'s K | V only, as a
+        one-entry list, in workspace buffers of its own (the seams run one block at a time; reusing the forward's buffers
+        would evict them and the graphs captured against them)."""
         C, D = self.dim, self.head_dim
         n_img = 257 if self.variant == "14b" else 0
         ctx_txt = ctx[n_img:]
+        ids = range(self.layers) if block is None else range(block, block + 1)
+        rows = slice(ids[0] * 2 * C, (ids[-1] + 1) * 2 * C)
+        tag = "_all" if block is None else "_one"
         alloc = (lambda key, shape: torch.empty(shape, device=self.device, dtype=_BF16)) if own_storage else \
             (lambda key, shape: self._buf(key, shape, _BF16))
-        kv_all = alloc("ckv_all", (ctx_txt.shape[0], self.layers * 2 * C))
-        ops.gemm(ctx_txt, self.cw_kv_all, self.cb_kv_all, kv_all, ops.YB_EPI_BF16)
+        kv_all = alloc("ckv" + tag, (ctx_txt.shape[0], len(ids) * 2 * C))
+        ops.gemm(ctx_txt, self.cw_kv_all[rows], self.cb_kv_all[rows], kv_all, ops.YB_EPI_BF16)
         kvi_all = None
         if n_img:
-            kvi_all = alloc("ckv_img_all", (n_img, self.layers * 2 * C))
-            ops.gemm(ctx[:n_img], self.cw_kv_img_all, self.cb_kv_img_all, kvi_all, ops.YB_EPI_BF16)
+            kvi_all = alloc("ckv_img" + tag, (n_img, len(ids) * 2 * C))
+            ops.gemm(ctx[:n_img], self.cw_kv_img_all[rows], self.cb_kv_img_all[rows], kvi_all, ops.YB_EPI_BF16)
         out = []
-        for i, b in enumerate(self.blocks):
-            kv = kv_all[:, i * 2 * C:(i + 1) * 2 * C]
+        for j, i in enumerate(ids):
+            b = self.blocks[i]
+            kv = kv_all[:, j * 2 * C:(j + 1) * 2 * C]
             ops.rmsnorm_rope(kv[:, :C], b["cnk"], None, D, self.eps)
             kvi = None
             if kvi_all is not None:
-                kvi = kvi_all[:, i * 2 * C:(i + 1) * 2 * C]
+                kvi = kvi_all[:, j * 2 * C:(j + 1) * 2 * C]
                 ops.rmsnorm_rope(kvi[:, :C], b["cnk_img"], None, D, self.eps)
             out.append((kv, kvi))
         return out
@@ -618,56 +624,54 @@ class WanDiT:
         return kv
 
     def _block(self, i: int, xs: Tensor, mod: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int,
-               ctx: Tensor, L_true: Optional[int] = None) -> None:
-        """One WanAttentionBlock in place on the fp32 residual stream xs [L, C] (a token shard under Ulysses)."""
-        if self._fp8:
-            return self._block_fp8(self.blocks[i], xs, mod[i], tok_idx, rope, rope_len,
-                                   ctx[i] if isinstance(ctx, list) else self._cross_kv(ctx)[i],
-                                   L_true if L_true is not None else xs.shape[0])
-        b, C, H, D = self.blocks[i], self.dim, self.heads, self.head_dim
+               ctx: List, L_true: Optional[int] = None) -> None:
+        """One WanAttentionBlock in place on the fp32 residual stream xs [L, C] (a token shard under Ulysses). mod: the
+        modulation tables [layers, U, 6, C]; ctx: every block's cross K|V (_cross_kv); L_true: rows that are self-attention
+        keys (default all)."""
+        self._block_body(i, xs, mod[i], tok_idx, rope, rope_len, ctx[i], L_true if L_true is not None else xs.shape[0])
+
+    def _block_body(self, i: int, xs: Tensor, m: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int, kv,
+                    k_len: int) -> None:
+        """Block i with its modulation rows m [U, 6, C] (shift_a, scale_a, gate_a, shift_f, scale_f, gate_f) and its cross
+        K|V `kv`."""
+        b, C, T = self.blocks[i], self.dim, self.timer
         L = xs.shape[0]
-        m = mod[i]                                             # [U, 6, C]: shift_a, scale_a, gate_a, shift_f, scale_f, gate_f
-        h = self._buf("h", (L, C), _BF16)
         qkv = self._buf("qkv", (L, 3 * C), _BF16)
         att = self._buf("att", (L, C), _BF16)
-        # --- self-attention ---
-        T = self.timer
         T.begin("ln_modulate")
-        ops.ln_modulate(xs, h, m[:, 1], m[:, 0], tok_idx, eps=self.eps)
+        h = self._norm(xs, m[:, 1], m[:, 0], tok_idx)
         T.end("ln_modulate")
         if self.sp_world > 1:
-            self._self_attention_sp(i, b, h, xs, m, tok_idx, rope, rope_len, L_true if L_true is not None else L)
+            self._self_attention_sp(i, b, h, xs, m, tok_idx, rope, rope_len, k_len)
         else:
-            self._self_attention_local(b, h, qkv, att, xs, m, tok_idx, rope, rope_len, L_true if L_true is not None else L)
-        self._cross_and_ffn(b, xs, h, qkv, att, m, tok_idx, ctx[i] if isinstance(ctx, list) else self._cross_kv(ctx)[i])
+            self._self_attention(b, h, qkv, att, rope, rope_len, k_len, xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
+        self._cross_and_ffn(b, xs, qkv, att, m, tok_idx, kv)
 
-    def _self_attention_local(self, b, h, qkv, att, xs, m, tok_idx, rope, rope_len, k_len) -> None:
-        """k_len: rows that are keys. All L on the 5B tree (wan23/modules/model.py:846-851); on the 14B regular-grid path
-        the reference passes k_lens = F*H*W, masking the zero-padded rows (wan/modules/model.py:311-314, 916)."""
-        C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
+    def _self_attention(self, b, a, qkv, att, rope, rope_len, k_len, out, epilogue, gate=None, tok_idx=None) -> None:
+        """q|k|v projection of the normed input `a`, RMSNorm + RoPE, attention, then the o projection into `out` (GATE_RES on
+        the residual stream, or BF16 for the self-attention seam). k_len: rows that are keys. All L on the 5B tree
+        (wan23/modules/model.py:846-851); on the 14B regular-grid path the reference passes k_lens = F*H*W, masking the
+        zero-padded rows (wan/modules/model.py:311-314, 916)."""
+        C, D, T = self.dim, self.head_dim, self.timer
         T.begin("gemm_qkv")
-        ops.gemm(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
+        self._linear(a, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
         T.end("gemm_qkv")
         T.begin("qk_norm_rope")
         ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, rope_len)
         T.end("qk_norm_rope")
         T.begin("self_attention")
-        if self.precision == "fp8_attn":
-            self._attention_fp8(qkv, att, k_len)
-        else:
-            ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
+        self._attention(qkv, att, k_len)
         T.end("self_attention")
         T.begin("gemm_o")
-        ops.gemm(att, b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
+        self._linear(self._quant(att, "att8"), b["w_o"], b["b_o"], out, epilogue, gate=gate, tok_idx=tok_idx)
         T.end("gemm_o")
 
-    def _cross_and_ffn(self, b, xs, h, qkv, att, m, tok_idx, ctx) -> None:
+    def _cross_and_ffn(self, b, xs, qkv, att, m, tok_idx, ctx) -> None:
         C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
-        L = xs.shape[0]
         # --- cross-attention (no gate, affine norm3) ---
-        ops.ln_modulate(xs, h, None, None, None, b["n3w"], b["n3b"], eps=self.eps)
+        h = self._norm(xs, None, None, None, b["n3w"], b["n3b"])
         q2 = qkv[:, :C]
-        ops.gemm(h, b["cw_q"], b["cb_q"], q2, ops.YB_EPI_BF16)
+        self._linear(h, b["cw_q"], b["cb_q"], q2, ops.YB_EPI_BF16)
         ops.rmsnorm_rope(q2, b["cnq"], None, D, self.eps)
         kv, kvi = ctx                                            # this block's normalised K | V (see _cross_kv)
         T.begin("cross_attention")
@@ -675,68 +679,72 @@ class WanDiT:
         T.end("cross_attention")
         if kvi is not None:
             ops.attention(q2, kvi[:, :C], kvi[:, C:], att, H, accumulate=True)
-        ops.gemm(att, b["cw_o"], b["cb_o"], xs, ops.YB_EPI_GATE_RES)
+        self._linear(self._quant(att, "att8"), b["cw_o"], b["cb_o"], xs, ops.YB_EPI_GATE_RES)
         # --- FFN ---
-        ops.ln_modulate(xs, h, m[:, 4], m[:, 3], tok_idx, eps=self.eps)
-        hid = self._buf("ffn_hid", (L, self.ffn_dim), _BF16)
+        h = self._norm(xs, m[:, 4], m[:, 3], tok_idx)
         T.begin("gemm_ffn1")
-        ops.gemm(h, b["w1"], b["b1"], hid, ops.YB_EPI_GELU_BF16)
+        hid = self._ffn0(h, b)
         T.end("gemm_ffn1")
         T.begin("gemm_ffn2")
-        ops.gemm(hid, b["w2"], b["b2"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 5], tok_idx=tok_idx)
+        self._linear(hid, b["w2"], b["b2"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 5], tok_idx=tok_idx)
         T.end("gemm_ffn2")
 
     # ------------------------------------------------------------------------------------------------------
-    # precision="fp8": the same block with e4m3 operands for the six converted linears (include/yume_b200_fp8.h)
+    # precision: the only places the block code branches on it. Under "fp8" an activation that feeds one of the FP8_WEIGHTS
+    # linears is an e4m3 (values, 1x128 scales) pair (include/yume_b200_fp8.h); "fp8_attn" also runs the self-attention in e4m3
     # ------------------------------------------------------------------------------------------------------
     def _act8(self, key: str, rows: int, cols: int) -> Tuple[Tensor, Tensor]:
         """Workspace of one fp8 activation: e4m3 values [rows, cols] and their 1x128 scales f32 [cols / 128, ld >= rows]."""
         return (self._buf(key + "_q", (rows, cols), torch.float8_e4m3fn),
                 self._buf(key + "_s", (cols // 128, ops.fp8_scale_ld(rows)), _F32))
 
-    def _block_fp8(self, b: dict, xs: Tensor, m: Tensor, tok_idx: Optional[Tensor], rope: Tensor, rope_len: int, ctx,
-                   k_len: int) -> None:
-        """One block (weights `b`, modulation rows m [U, 6, C], this block's cross K|V `ctx`) in place on xs [L, C]."""
-        C = self.dim
-        L = xs.shape[0]
-        h8 = self._act8("h8", L, C)
-        qkv = self._buf("qkv", (L, 3 * C), _BF16)
-        att = self._buf("att", (L, C), _BF16)
-        T = self.timer
-        T.begin("ln_modulate")
-        ops.ln_modulate_fp8(xs, *h8, m[:, 1], m[:, 0], tok_idx, eps=self.eps)
-        T.end("ln_modulate")
-        self._self_attention_fp8(b, h8, qkv, att, rope, rope_len, k_len, xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
-        self._cross_and_ffn_fp8(b, xs, qkv, att, m, tok_idx, ctx)
+    def _norm(self, xs: Tensor, scale, shift, tok_idx, weight=None, bias=None):
+        """LayerNorm of xs (affine with weight, bias; modulated with scale, shift) as the next linear's input: bf16 `h`,
+        or the e4m3 pair `h8`."""
+        L, C = xs.shape
+        if self._fp8:
+            h8 = self._act8("h8", L, C)
+            ops.ln_modulate_fp8(xs, *h8, scale, shift, tok_idx, weight, bias, eps=self.eps)
+            return h8
+        h = self._buf("h", (L, C), _BF16)
+        ops.ln_modulate(xs, h, scale, shift, tok_idx, weight, bias, eps=self.eps)
+        return h
 
-    def _self_attention_fp8(self, b, h8, qkv, att, rope, rope_len, k_len, out, epilogue, gate=None, tok_idx=None) -> None:
-        """q|k|v projection of the quantised input h8, RMSNorm + RoPE, attention, then the attention output quantised per 1x128
-        group and projected by o into `out` (GATE_RES on the residual stream, or BF16 for the self-attention seam)."""
-        C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
-        L = qkv.shape[0]
-        T.begin("gemm_qkv")
-        ops.gemm_fp8(*h8, *b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
-        T.end("gemm_qkv")
-        T.begin("qk_norm_rope")
-        ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, rope_len)
-        T.end("qk_norm_rope")
-        T.begin("self_attention")
-        if self.precision == "fp8_attn":
-            self._attention_fp8(qkv, att, k_len)
+    def _quant(self, x: Tensor, key: str):
+        """A bf16 activation as the next linear's input: x itself, or x quantised per 1x128 group into the pair `key`."""
+        if not self._fp8:
+            return x
+        x8 = self._act8(key, *x.shape)
+        ops.quant_rows_fp8(x, *x8)
+        return x8
+
+    def _linear(self, a, w, bias, out, epilogue, gate=None, tok_idx=None) -> None:
+        """One of the FP8_WEIGHTS block linears on an input from _norm / _quant / _ffn0."""
+        if self._fp8:
+            ops.gemm_fp8(*a, *w, bias, out, epilogue, gate=gate, tok_idx=tok_idx)
         else:
-            ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
-        T.end("self_attention")
-        T.begin("gemm_o")
-        a8 = self._act8("att8", L, C)
-        ops.quant_rows_fp8(att, *a8)
-        ops.gemm_fp8(*a8, *b["w_o"], b["b_o"], out, epilogue, gate=gate, tok_idx=tok_idx)
-        T.end("gemm_o")
+            ops.gemm(a, w, bias, out, epilogue, gate=gate, tok_idx=tok_idx)
 
-    def _attention_fp8(self, qkv: Tensor, att: Tensor, k_len: int) -> None:
-        """precision="fp8_attn": self-attention of the normed, roped q|k|v rows on e4m3 operands (include/yume_b200_fp8_attn.h).
-        q and k are quantised by one launch over the [L, 2C] view (a 1x128 group is one head of one token: q scales of head h
-        at scale row h, k scales at heads + h), v transposed per (head, 128-key tile); out bf16 `att`."""
+    def _ffn0(self, h, b: dict):
+        """ffn.0 + GELU of the normed input h, as ffn.2's input: bf16 `ffn_hid`, or the e4m3 pair `ffn_hid8` that the GEMM's
+        epilogue quantises."""
+        if self._fp8:
+            hid = self._act8("ffn_hid8", h[0].shape[0], self.ffn_dim)
+            ops.gemm_fp8(*h, *b["w1"], b["b1"], hid[0], ops.YB_EPI_GELU_FP8, out_scale=hid[1])
+            return hid
+        hid = self._buf("ffn_hid", (h.shape[0], self.ffn_dim), _BF16)
+        ops.gemm(h, b["w1"], b["b1"], hid, ops.YB_EPI_GELU_BF16)
+        return hid
+
+    def _attention(self, qkv: Tensor, att: Tensor, k_len: int) -> None:
+        """Self-attention of the normed, roped q|k|v rows over the first k_len rows as keys, into bf16 `att`. "fp8_attn" runs
+        it on e4m3 operands (include/yume_b200_fp8_attn.h): q and k are quantised by one launch over the [L, 2C] view (a 1x128
+        group is one head of one token: q scales of head h at scale row h, k scales at heads + h), v transposed per (head,
+        128-key tile)."""
         C, H = self.dim, self.heads
+        if self.precision != "fp8_attn":
+            ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
+            return
         L = qkv.shape[0]
         Lkp = ops.vt8_keys(k_len)
         qk8, qk_s = self._act8("qk8", L, 2 * C)
@@ -745,32 +753,6 @@ class WanDiT:
         ops.quant_rows_fp8(qkv[:, :2 * C], qk8, qk_s)
         ops.quant_vt_fp8(qkv[:k_len, 2 * C:], vt8, v_s, H)
         ops.attention_fp8(qk8[:, :C], qk8[:k_len, C:], qk_s, vt8, v_s, att, H)
-
-    def _cross_and_ffn_fp8(self, b, xs, qkv, att, m, tok_idx, ctx) -> None:
-        C, H, D, T = self.dim, self.heads, self.head_dim, self.timer
-        L = xs.shape[0]
-        h8 = self._act8("h8", L, C)
-        ops.ln_modulate_fp8(xs, *h8, None, None, None, b["n3w"], b["n3b"], eps=self.eps)
-        q2 = qkv[:, :C]
-        ops.gemm_fp8(*h8, *b["cw_q"], b["cb_q"], q2, ops.YB_EPI_BF16)
-        ops.rmsnorm_rope(q2, b["cnq"], None, D, self.eps)
-        kv, kvi = ctx
-        T.begin("cross_attention")
-        ops.attention(q2, kv[:, :C], kv[:, C:], att, H)
-        T.end("cross_attention")
-        if kvi is not None:
-            ops.attention(q2, kvi[:, :C], kvi[:, C:], att, H, accumulate=True)
-        a8 = self._act8("att8", L, C)
-        ops.quant_rows_fp8(att, *a8)
-        ops.gemm_fp8(*a8, *b["cw_o"], b["cb_o"], xs, ops.YB_EPI_GATE_RES)
-        ops.ln_modulate_fp8(xs, *h8, m[:, 4], m[:, 3], tok_idx, eps=self.eps)
-        hid8 = self._act8("ffn_hid8", L, self.ffn_dim)
-        T.begin("gemm_ffn1")
-        ops.gemm_fp8(*h8, *b["w1"], b["b1"], hid8[0], ops.YB_EPI_GELU_FP8, out_scale=hid8[1])
-        T.end("gemm_ffn1")
-        T.begin("gemm_ffn2")
-        ops.gemm_fp8(*hid8, *b["w2"], b["b2"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 5], tok_idx=tok_idx)
-        T.end("gemm_ffn2")
 
     def weight_bytes(self) -> int:
         """Bytes of every weight tensor the engine holds on its device (bench and tests compare the two precisions)."""
@@ -792,22 +774,6 @@ class WanDiT:
                 continue
             add(v)
         return total
-
-    def _cross_kv_one(self, i: int, ctx: Tensor):
-        """Block i's cross-attention K | V only (the block / self-attention seams run one block at a time)."""
-        C, D = self.dim, self.head_dim
-        n_img = 257 if self.variant == "14b" else 0
-        ctx_txt = ctx[n_img:]
-        kv = self._buf("ckv_one", (ctx_txt.shape[0], 2 * C), _BF16)
-        ops.gemm(ctx_txt, self.cw_kv_all[i * 2 * C:(i + 1) * 2 * C], self.cb_kv_all[i * 2 * C:(i + 1) * 2 * C], kv, ops.YB_EPI_BF16)
-        ops.rmsnorm_rope(kv[:, :C], self.blocks[i]["cnk"], None, D, self.eps)
-        kvi = None
-        if n_img:
-            kvi = self._buf("ckv_img_one", (n_img, 2 * C), _BF16)
-            ops.gemm(ctx[:n_img], self.cw_kv_img_all[i * 2 * C:(i + 1) * 2 * C], self.cb_kv_img_all[i * 2 * C:(i + 1) * 2 * C], kvi,
-                     ops.YB_EPI_BF16)
-            ops.rmsnorm_rope(kvi[:, :C], self.blocks[i]["cnk_img"], None, D, self.eps)
-        return kv, kvi
 
     def rope_from_reference(self, freqs: Tensor, grid: Optional[Sequence[int]], packed: bool) -> Tuple[Tensor, int]:
         """(cos, sin) table + number of rotated rows from what the reference hands its blocks: on the FramePack path `freqs`
@@ -839,18 +805,9 @@ class WanDiT:
             mod = ops.bcast_add(self.block_mod[i:i + 1], e0).view(1, e0.shape[0], 6, C)
             rope, rope_len = self.rope_from_reference(freqs, grid, packed) if (packed or freqs is not None) else \
                 (self._rope_table([(grid[0], grid[1], grid[2], 0)]), grid[0] * grid[1] * grid[2])
-            ctx = self._cross_kv_one(i, context.to(device=self.device, dtype=_BF16).contiguous())
-            b = self.blocks[i]
-            m = mod[0]
-            if self._fp8:
-                self._block_fp8(b, xs, m, tok_idx, rope, min(rope_len, L), ctx, L if k_len is None else int(k_len))
-                return xs
-            h = self._buf("h", (L, C), _BF16)
-            qkv = self._buf("qkv", (L, 3 * C), _BF16)
-            att = self._buf("att", (L, C), _BF16)
-            ops.ln_modulate(xs, h, m[:, 1], m[:, 0], tok_idx, eps=self.eps)
-            self._self_attention_local(b, h, qkv, att, xs, m, tok_idx, rope, min(rope_len, L), L if k_len is None else int(k_len))
-            self._cross_and_ffn(b, xs, h, qkv, att, m, tok_idx, ctx)
+            kv = self._cross_kv(context.to(device=self.device, dtype=_BF16).contiguous(), block=i)[0]
+            with self.sequence_parallel_disabled():           # one sample on this GPU, also under Ulysses
+                self._block_body(i, xs, mod[0], tok_idx, rope, min(rope_len, L), kv, L if k_len is None else int(k_len))
         return xs
 
     @torch.no_grad()
@@ -859,27 +816,17 @@ class WanDiT:
         """`WanSelfAttention.forward` seam for one sample: x [L, C] (the modulated, normalised input) -> o(attention(...)) as
         bf16 [L, C] — q/k/v projection, RMSNorm(q), RMSNorm(k), RoPE, attention, output projection; no gate, no residual
         (wan23/modules/model.py:178-207)."""
-        C, H, D = self.dim, self.heads, self.head_dim
+        C = self.dim
         with torch.cuda.device(self.device):
             h = x.to(device=self.device, dtype=_BF16).contiguous()
             L = h.shape[0]
-            b = self.blocks[i]
             rope, rope_len = self.rope_from_reference(freqs, grid, packed)
             qkv = self._buf("qkv", (L, 3 * C), _BF16)
             att = self._buf("att", (L, C), _BF16)
-            if self._fp8:
-                h8 = self._act8("h8", L, C)
-                ops.quant_rows_fp8(h, *h8)
-                out = torch.empty(L, C, device=self.device, dtype=_BF16)
-                self._self_attention_fp8(b, h8, qkv, att, rope, min(rope_len, L), L if k_len is None else int(k_len), out,
-                                         ops.YB_EPI_BF16)
-                return out
-            ops.gemm(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
-            ops.qk_norm_rope(qkv[:, :C], qkv[:, C:2 * C], b["nq"], b["nk"], rope, D, self.eps, min(rope_len, L))
-            kl = L if k_len is None else int(k_len)
-            ops.attention(qkv[:, :C], qkv[:kl, C:2 * C], qkv[:kl, 2 * C:], att, H)
+            a = self._quant(h, "h8")
             out = torch.empty(L, C, device=self.device, dtype=_BF16)
-            ops.gemm(att, b["w_o"], b["b_o"], out, ops.YB_EPI_BF16)
+            self._self_attention(self.blocks[i], a, qkv, att, rope, min(rope_len, L), L if k_len is None else int(k_len), out,
+                                 ops.YB_EPI_BF16)
         return out
 
     # ------------------------------------------------------------------------------------------------------
