@@ -14,8 +14,10 @@ pytestmark = pytest.mark.gpu
 # one block at the real 5B / 14B width 2.6e-2 (vs the fp32 oracle 5.3e-2)
 QDQ_TOL = 3e-2
 
+# wan21_h8:14b_grid_padded is the one case with k_len < L: seq_len 112 over 105 keys, the zero padding rows masked as keys
 CASES = [("wan23_tiny.pt", "5b_pack_h10"), ("wan23_tiny.pt", "5b_grid_padded"), ("wan21_tiny.pt", "14b_pack_h4"),
-         ("wan21_tiny.pt", "14b_grid"), ("wan23_h8.pt", "5b_pack_h10"), ("wan21_h8.pt", "14b_pack_lfz8")]
+         ("wan21_tiny.pt", "14b_grid"), ("wan23_h8.pt", "5b_pack_h10"), ("wan21_h8.pt", "14b_pack_lfz8"),
+         ("wan21_h8.pt", "14b_grid_padded")]
 
 
 def _inputs(cfg, c):

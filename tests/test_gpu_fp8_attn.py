@@ -1,5 +1,5 @@
-"""End to end of WanDiT(precision="fp8_attn") on the H100: against the fp8-attention oracle (oracle/fp8_attn.py) on the six goldens
-of tests/test_gpu_fp8.py, one block at the real 5B and 14B width against that oracle and the fp32 oracle, and eager, context-cache
+"""End to end of WanDiT(precision="fp8_attn") on the H100: against the fp8-attention oracle (oracle/fp8_attn.py) on the goldens of
+tests/test_gpu_fp8.py, one block at the real 5B and 14B width against that oracle and the fp32 oracle, and eager, context-cache
 and graph-replay runs bit-identical to each other."""
 import pytest
 import torch

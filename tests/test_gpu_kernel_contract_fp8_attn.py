@@ -32,9 +32,12 @@ def attention_fp8_bound(q, k, v, scale, nkv, ns=1):
     ref = softmax(q k^T scale) v. With p the exact probabilities and l = sum_j exp(s_j - max s):
       logits      e = 4 2^-ACC_BITS scale (|q| |k|^T)  (four truncating k32 steps of the S wgmma) + 4 u32 |s|  (k scale, row
                   factor, exp2 argument); a logit error e moves the output by at most 2 e (p |v|)
-      P8          round-to-nearest e4m3 of 256 p against the running max: relative error <= 2^-4 per key, independent and
-                  zero-mean, so their sum is bounded by Z_P standard deviations, Z_P 2^-4 / sqrt(3) sqrt(p^2 |v|^2); subnormal P8
-                  (and P8 flushed to 0) add at most 2^-18 per key: 2^-18 sum_j |v_j| / l
+      P8          round-to-nearest e4m3 of 256 p against the running max: relative error <= 2^-4 per key, zero-mean and
+                  independent between distinct keys, so their sum is bounded by Z_P standard deviations,
+                  Z_P 2^-4 / sqrt(3) sqrt(sum_g (p_g |v_g|)^2); keys with identical (k, v) rows round alike (the zero padding
+                  rows of a padded 5B grid are keys, and after a block they are all the same row), so each group g of them
+                  counts as one key holding their summed p_g; subnormal P8 (and P8 flushed to 0) add at most 2^-18 per key:
+                  2^-18 sum_j |v_j| / l
       O_tile      four truncating k32 steps per tile: 4 2^-ACC_BITS (1 + 2^-4) (p |v|)
       fp32        promotion, alpha, l and the combine as attention_bound_prod counts them: (26 nkv + 36 + 3 ns) u32 (p |v|)
       output      bf16 rounding U16 |ref|"""
@@ -44,7 +47,10 @@ def attention_fp8_bound(q, k, v, scale, nkv, ns=1):
     pv = p @ v.abs()
     e = (4 * 2.0 ** -ACC_BITS * scale * (q.abs() @ k.abs().t()) + 4 * U32 * s.abs()).amax(dim=-1, keepdim=True)
     l = torch.exp(s - s.amax(dim=-1, keepdim=True)).sum(dim=-1, keepdim=True)
-    stat = Z_P * P_REL / math.sqrt(3.0) * torch.sqrt((p * p) @ (v * v))
+    rows, group = torch.unique(torch.cat([k, v], dim=1), dim=0, return_inverse=True)
+    pg = torch.zeros(p.shape[0], rows.shape[0], dtype=p.dtype, device=p.device).index_add_(1, group, p)
+    vg = rows[:, k.shape[1]:]
+    stat = Z_P * P_REL / math.sqrt(3.0) * torch.sqrt((pg * pg) @ (vg * vg))
     sub = P_SUB * v.abs().sum(dim=0, keepdim=True) / l
     extra = (26 * nkv + 36 + (3 * ns if ns > 1 else 0)) * U32 + 4 * 2.0 ** -ACC_BITS * (1 + P_REL)
     return ref, U16 * ref.abs() + (2 * e + extra) * pv + stat + sub
