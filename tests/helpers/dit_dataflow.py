@@ -1,10 +1,15 @@
-"""TEST INFRASTRUCTURE: the WanDiT block checked launch by launch.
+"""TEST INFRASTRUCTURE: the WanDiT forward checked launch by launch.
 
-A SPEC states the dataflow of one Wan block (and of the cross-attention K|V launches in front of it) independently of
-yume_b200/dit.py, from the reference's WanAttentionBlock (wan23/modules/model.py:272-316, wan/modules/model.py:444-496, as
-oracle/wan_dit.py restates it): an ordered list of stages, each naming its ops entry, where every operand must come from (an
-earlier stage's output, a weight rebuilt from the reference's state-dict keys, a modulation row with its token index, RoPE rows
-from oracle.wan_dit.grid_freqs, the first k_len rows) and which per-element bound its output must meet.
+A SPEC states the dataflow of one forward independently of yume_b200/dit.py, from the reference's WanModel.forward
+(wan23/modules/model.py:547-865, wan/modules/model.py:723-1013, as oracle/wan_dit.py restates it): an ordered list of stages in
+six phases (embed: the FramePack segments of WanOracle._segments or the grid, each a patchify + GEMM; time: the sinusoid, the
+time MLP and projection, the block and head tables, per 16-row chunk; context: the text MLP and the 14B image MLP; cross_kv; one
+WanAttentionBlock; head: the modulated LayerNorm, the head linear, unpatchify of the new frames). Each stage names its ops entry,
+where every operand must come from (an earlier stage's output, a weight rebuilt from the reference's state-dict keys, the
+forward's own inputs in the reference's token layout, a modulation row with its token index, RoPE rows from
+oracle.wan_dit.grid_freqs, the first k_len rows) and which per-element bound its output must meet. At the first block's entry the
+whole residual stream must equal the embed GEMMs' outputs row for row in the reference's token order, with exact zeros on the
+padding rows, and each token's index must point at the table row of its own timestep.
 
 A CHECKER sits between the engine and its ops module (`dit.ops`). Outside a checked region it only passes launches through;
 inside one it takes the next stage for every launch and checks
@@ -12,9 +17,13 @@ inside one it takes the next stage for every launch and checks
   inputs   every operand is torch.equal to the source the stage names (view shape, row count, scale table included);
   output   right after the launch, against an fp64 recomputation from those inputs within the kernel's contract bound
            (tests/test_gpu_kernel_contract*.py: gemm_epilogue_ref / gemm_bounds, _ln_ref, _rr_ref, attention_bound_prod,
-           the fp8 gemm_bound, attention_fp8_bound; the fp8 quantisers bit-identical to their twins in oracle/fp8*.py).
-Only the snapshots a later stage reads are kept, and each is dropped after its last reader, so production L fits. Large
-launches are sampled like the production contract (gemm_sample rows and columns, attention_sample rows).
+           the fp8 gemm_bound, attention_fp8_bound, sinusoidal_ref, linear_f32_small_ref, linear_f32_ref; the fp8
+           quantisers bit-identical to their twins in oracle/fp8*.py; patchify, unpatchify and bcast_add bit-identical to the
+           torch stand-ins' reshapes and the fp32 add).
+Only the snapshots a later stage (or the block-entry check) reads are kept, and each is dropped after its last reader, so
+production L fits. Large launches are sampled like the production contract (gemm_sample rows and columns, attention_sample
+rows). The geometry comes from WanOracle._segments, the convpadd shapes and grid_freqs, never from the oracle's CPU pack (its
+real-width conv3d is far too slow at production sizes).
 
 The same spec and checker run on the H100 (tests/test_gpu_dit_dataflow.py) and over the torch stand-ins at tiny width on the
 CPU (tests/test_dit_dataflow_cpu.py), where wiring defects are patched into the engine and must be caught."""
@@ -29,9 +38,11 @@ from typing import Callable, Dict, List, Optional
 import torch
 
 import test_gpu_kernel_contract as KC
+import test_gpu_kernel_contract_ext as KE
 import test_gpu_kernel_contract_fp8 as K8
 import test_gpu_kernel_contract_fp8_attn as KA
 import test_gpu_kernel_contract_prod as KP
+from helpers import torch_ops as TO
 from oracle import synth
 from oracle.fp8 import dequantize_act, quantize_act, quantize_weight
 from oracle.fp8_attn import dequantize_vt, quantize_vt
@@ -41,9 +52,12 @@ from yume_b200 import ops as _real_ops
 D = 128                       # head_dim of both trees
 EPS = 1e-6
 ENTRIES = ("gemm", "gemm_fp8", "ln_modulate", "ln_modulate_fp8", "qk_norm_rope", "rmsnorm_rope", "quant_rows_fp8",
-           "quant_vt_fp8", "attention", "attention_fp8")
+           "quant_vt_fp8", "attention", "attention_fp8", "patchify", "sinusoidal", "linear_f32_small", "bcast_add", "linear_f32",
+           "unpatchify")
 SIGS = {e: inspect.signature(getattr(_real_ops, e)) for e in ENTRIES}
-EPI = dict(BF16=0, GELU=1, F32=2, GATE_RES=3, GELU_FP8=8)     # include/yume_b200.h, include/yume_b200_fp8.h
+EPI = dict(BF16=0, GELU=1, F32=2, GATE_RES=3, GELU_ERF=4, GELU_FP8=8)     # include/yume_b200.h, include/yume_b200_fp8.h
+IMG_EPS = 1e-5                # MLPProj's LayerNorms (nn.LayerNorm default, wan/modules/model.py:533-537)
+T_CHUNK = 16                  # timestep rows per time-table launch chain (yb_linear_f32_small's M limit)
 FULL_ROWS = 1024              # launches with at most this many rows are checked on every row, larger ones sampled
 
 
@@ -61,12 +75,16 @@ class Src:
     reads: tuple = ()          # stage names whose snapshots this source reads
 
 
-def S(stage, part="", rows=None, cols=None, kind="tensor"):
-    rs = slice(None) if rows is None else slice(0, rows)
+def S(stage, part="", rows=None, cols=None, kind="tensor", fn=None, what=""):
+    """Stage `stage`'s output (part `part`), rows [:rows] (or [lo:hi] for a pair), columns [c0:c1], then `fn` (a view)."""
+    rows = None if rows is None else (rows if isinstance(rows, tuple) else (0, rows))
+    rs = slice(None) if rows is None else slice(*rows)
     cs = slice(None) if cols is None else slice(*cols)
-    label = f"{stage}{'.' + part if part else ''}" + (f"[:{rows}]" if rows is not None else "") + \
-        (f"[:, {cols[0]}:{cols[1]}]" if cols is not None else "")
-    return Src(label, lambda ck: ck.snap[stage][part][rs, cs], kind, (stage,))
+    label = f"{stage}{'.' + part if part else ''}" + \
+        (f"[{rows[0] or ''}:{'' if rows[1] is None else rows[1]}]" if rows is not None else "") + \
+        (f"[:, {cols[0]}:{cols[1]}]" if cols is not None else "") + (f" {what}" if what else "")
+    f = fn or (lambda t: t)
+    return Src(label, lambda ck: f(ck.snap[stage][part][rs, cs]), kind, (stage,))
 
 
 def CAT(*srcs):
@@ -130,7 +148,9 @@ class Checker:
         self.pos, self.stop, self.phase = 0, 0, None
         self.worst: Dict[str, float] = {}
         self.stream = None                  # the residual stream the last pass-through GATE_RES launch wrote
-        self.env: Dict[str, torch.Tensor] = {}   # what the run hands the block: x_in, ctx, mod (filled by Cell's wrappers)
+        self.env: Dict[str, torch.Tensor] = {}   # what the run hands the block: x_in (and for the seams ctx, mod)
+        self.pinned: set = set()            # stages whose snapshots the block-entry check reads (kept until unpin)
+        self.entered: List[str] = []        # phases in the order they were opened
         self.proxy = _Proxy(self)
 
     # ---- program -----------------------------------------------------------------------------------------------
@@ -144,19 +164,39 @@ class Checker:
                 for r in src.reads:
                     self.last_read[r] = j
 
-    @contextlib.contextmanager
-    def region(self, phase):
-        """Launches inside are the stages of `phase`, exactly as many as it has."""
+    def enter(self, phase):
+        """Close the open phase (it must have made all its launches) and open `phase`: launches from here on are its stages."""
+        self.leave()
         rg = self.phases[phase]
-        assert self.phase is None, f"{self.tag}: region {phase} opened inside {self.phase}"
         self.phase, self.pos, self.stop = phase, rg.start, rg.stop
-        try:
-            yield
-        finally:
-            ended, self.phase = self.pos, None
+        self.entered.append(phase)
+
+    def leave(self):
+        """Close the open phase, if any: it must have made exactly the spec's number of launches."""
+        if self.phase is None:
+            return
+        phase, rg, ended = self.phase, self.phases[self.phase], self.pos
+        self.phase = None
         if ended != rg.stop:
             raise AssertionError(f"{self.tag}: {phase} made {ended - rg.start} launches, the spec has {len(rg)}: stage "
                                  f"'{self.program[ended].name}' ({self.program[ended].entry}) never ran")
+
+    @contextlib.contextmanager
+    def region(self, phase):
+        """Launches inside are the stages of `phase`, exactly as many as it has."""
+        assert self.phase is None, f"{self.tag}: region {phase} opened inside {self.phase}"
+        self.enter(phase)
+        try:
+            yield
+        except BaseException:
+            self.phase = None
+            raise
+        self.leave()
+
+    def unpin(self):
+        for name in self.pinned:
+            self.snap.pop(name, None)
+        self.pinned = set()
 
     # ---- one launch ----------------------------------------------------------------------------------------------
     def launch(self, entry, a, k):
@@ -183,14 +223,15 @@ class Checker:
         out = fn(*a, **k)
         if self.base is _real_ops:
             torch.cuda.synchronize()
-        keep = st.name in self.last_read and self.last_read[st.name] > self.pos
+        args["ret"] = out                   # the entries that allocate their output (sinusoidal, linear_f32_small, bcast_add)
+        keep = (st.name in self.last_read and self.last_read[st.name] > self.pos) or st.name in self.pinned
         if keep:
             self.snap[st.name] = {part: f(args).clone() for part, f in st.outputs.items()}
         if st.check is not None:
             w = st.check(self, st, args, inp)
             self.worst[st.name] = max(self.worst.get(st.name, 0.0), w)
         del inp
-        for name in [n for n in self.snap if self.last_read.get(n, -1) <= self.pos]:
+        for name in [n for n in self.snap if self.last_read.get(n, -1) <= self.pos and n not in self.pinned]:
             del self.snap[name]
         self.pos += 1
         return out
@@ -268,15 +309,24 @@ def _mod_rows(t, tok, rows):
     return t.double()[idx]
 
 
+def _shape(ck, st, param, t, want):
+    if tuple(t.shape) != tuple(want):
+        raise AssertionError(f"{ck.tag}: stage '{st.name}' operand '{param}' has shape {tuple(t.shape)}, the spec's is "
+                             f"{tuple(want)}")
+
+
 def check_ln(ck, st, a, inp):
+    """_ln_ref on every row, into bf16 (bf16_out_bound) or f32 (the head)."""
     x, out, tok = inp["x"], a["out"], inp["tok_idx"]
     L, C = x.shape
+    _shape(ck, st, "out", out, (L, C))
     worst = 0.0
     for r0 in range(0, L, 4096):
         rows = torch.arange(r0, min(L, r0 + 4096), device=x.device)
-        y, f32 = KC._ln_ref(x[rows], C, EPS, inp["weight"], inp["bias"], _mod_rows(inp["scale"], tok, rows),
+        y, f32 = KC._ln_ref(x[rows], C, inp["eps"], inp["weight"], inp["bias"], _mod_rows(inp["scale"], tok, rows),
                             _mod_rows(inp["shift"], tok, rows))
-        worst = max(worst, _ratio(out[rows], y, KC.bf16_out_bound(y, f32), f"{ck.tag}: stage '{st.name}' output"))
+        bound = f32 if out.dtype == torch.float32 else KC.bf16_out_bound(y, f32)
+        worst = max(worst, _ratio(out[rows], y, bound, f"{ck.tag}: stage '{st.name}' output"))
     return worst
 
 
@@ -343,9 +393,10 @@ def check_gemm(ck, st, a, inp):
     per 64-column band (gemm_sample)."""
     A, B, bias, epi = inp["a"], inp["w"], inp["bias"], inp["epilogue"]
     M, N = A.shape[0], B.shape[0]
+    out = a["out"]
+    _shape(ck, st, "out", out, (M, N))
     rows, cols = _rows(M, (ck.tag, st.name)).to(A.device), _cols(N, (ck.tag, st.name)).to(A.device)
     (accR, FR), (accC, FC) = KP.gemm_ref_rows_cols(A, B, rows, cols)
-    out = a["out"]
     worst = 0.0
     allr = torch.arange(M, device=A.device)
     for rr, cc, acc, Fb in ((rows, None, accR, FR), (allr, cols, accC, FC)):
@@ -386,6 +437,59 @@ def check_gemm8(ck, st, a, inp):
         ref = inp["out"][rows].double() + ref * gt
         bound = bound * gt.abs() + 2.0 ** -24 * ref.abs()
     return _ratio(a["out"][rows], ref, bound, what)
+
+
+def _exact(ck, st, got, want, what="output"):
+    if got.shape != want.shape or not torch.equal(got, want.to(got.device)):
+        n = int((got != want.to(got.device)).sum()) if got.shape == want.shape else got.numel()
+        raise AssertionError(f"{ck.tag}: stage '{st.name}' {what}: {n} of {got.numel()} elements differ from the spec's "
+                             f"{tuple(want.shape)} (bit-exact entry)")
+    return 0.0
+
+
+def check_patchify(ck, st, a, inp):
+    """Columns [0, Cin*ph*pw) bit-identical to the stand-in's reshape (zero fill past H, W: convpadd); the K padding columns the
+    GEMM also reads must be zero."""
+    x, out, ph, pw = inp["x"], a["out"], inp["ph"], inp["pw"]
+    Cin, Fr, H, W = x.shape
+    n, kc = Fr * -(-H // ph) * -(-W // pw), Cin * ph * pw
+    if out.shape[0] != n or out.shape[1] < kc:
+        raise AssertionError(f"{ck.tag}: stage '{st.name}' operand 'out' is {tuple(out.shape)} for {n} tokens of {kc} columns")
+    _exact(ck, st, out[:, :kc], TO.patchify(x, torch.empty(n, kc, dtype=torch.bfloat16, device=x.device), ph, pw))
+    return _exact(ck, st, out[:, kc:], torch.zeros_like(out[:, kc:]), "K padding columns")
+
+
+def check_sin(ck, st, a, inp):
+    ref, bound = KE.sinusoidal_ref(inp["t"], inp["dim"])
+    _shape(ck, st, "out", a["ret"], ref.shape)
+    return _ratio(a["ret"], ref, bound, f"{ck.tag}: stage '{st.name}' output")
+
+
+def check_lfs(ck, st, a, inp):
+    ref, bound = KE.linear_f32_small_ref(inp["x"], inp["w"], inp["bias"], inp["silu_in"])
+    _shape(ck, st, "out", a["ret"], ref.shape)
+    return _ratio(a["ret"], ref, bound, f"{ck.tag}: stage '{st.name}' output")
+
+
+def check_bcast(ck, st, a, inp):
+    return _exact(ck, st, a["ret"], inp["a"][:, None] + inp["b"][None])
+
+
+def check_lin32(ck, st, a, inp):
+    """linear_f32_ref on every row of a small launch, else on gemm_sample's rows."""
+    x, out = inp["x"], a["out"]
+    M, N = x.shape[0], inp["w"].shape[0]
+    _shape(ck, st, "out", out, (M, N))
+    rows = _rows(M, (ck.tag, st.name)).to(x.device)
+    ref, bound = KE.linear_f32_ref(x[rows], inp["w"], inp["bias"])
+    return _ratio(out[rows], ref, bound, f"{ck.tag}: stage '{st.name}' output")
+
+
+def check_unpatchify(ck, st, a, inp):
+    out, y = a["out"], inp["y"]
+    Fr, Hp, Wp, ph, pw = (inp[p] for p in ("F", "Hp", "Wp", "ph", "pw"))
+    _shape(ck, st, "out", out, (y.shape[1] // (ph * pw), Fr, Hp * ph, Wp * pw))
+    return _exact(ck, st, out, TO.unpatchify(y, torch.empty(out.shape, device=y.device), Fr, Hp, Wp, ph, pw))
 
 
 def _att_rows(Lq, H, key):
@@ -451,6 +555,45 @@ class Geometry:
     rope: torch.Tensor              # (cos, sin) f32 [R, 64, 2] of the rotated rows (rope_rows of grid_freqs)
     tok: Optional[torch.Tensor]     # int32 [L]: the modulation row of every token, or None (one row for all)
     kv_col: int = 0                 # position of the block among the blocks of the cross K|V GEMM
+    layout: Optional["Layout"] = None   # the whole forward (None: a seam, whose context and modulation rows the caller hands in)
+
+
+@dataclass
+class Segment:
+    """One patch-embedded piece of the token sequence: frames [f0, f1) of the input, the embedder and its patch, whether
+    patch_embedding_2x_f runs first, and the token grid (f, h, w) it yields at rows [row0, row0 + f*h*w)."""
+    f0: int
+    f1: int
+    name: str
+    patch: int
+    pre_2x_f: bool
+    crop: bool                      # plain Conv3d (patch_embedding): odd H / W lose their last row / column; else convpadd
+    grid: tuple
+    row0: int
+
+    @property
+    def n(self):
+        return math.prod(self.grid)
+
+
+@dataclass
+class Layout:
+    """The reference's token layout of one forward (from WanOracle._segments, convpadd shapes and grid_freqs) and its inputs on
+    the device."""
+    x: torch.Tensor                 # f32 [in_dim, F, H, W] (y concatenated on 14B)
+    segs: List[Segment]
+    L: int                          # rows of the residual stream (seq_len on the grid path)
+    n_real: int                     # rows the embedders write; the rest are zero padding tokens
+    L_hist: int                     # history tokens in front of the new frames' grid
+    grid: tuple                     # token grid of the new frames
+    t_rows: List[float]             # the timestep of each table row, in row order
+    context: torch.Tensor           # [S, text_dim] as the caller passed it
+    clip: Optional[torch.Tensor]    # [257, clip_dim] (14B)
+    layers: int = 0
+
+    @property
+    def t_chunks(self):
+        return [min(T_CHUNK, len(self.t_rows) - s) for s in range(0, len(self.t_rows), T_CHUNK)]
 
 
 def _w(sd, names, dev):
@@ -530,8 +673,25 @@ def _quant_stage(name, x):
                  check_q8)
 
 
-def _mod(j):
+def _table(lay, kind, j, i=None):
+    """Row j of the block-i modulation table (kind 'mod', [U, 6, C] rows) or of the head table (kind 'head', [U, 2, C]): the
+    time phase's bcast_add outputs of every 16-row chunk, concatenated along the timestep rows."""
+    names = [f"time[{c}].{kind}" for c in range(len(lay.t_chunks))]
+
+    def get(ck):
+        parts = []
+        for n, u in zip(names, lay.t_chunks):
+            t = ck.snap[n][""]
+            parts.append(t.view(lay.layers, u, 6, -1)[i] if kind == "mod" else t.view(u, 2, -1))
+        return torch.cat(parts, 0)[:, j]
+    return Src(f"{kind} table row {j}" + (f" of block {i}" if i is not None else "") + f" ({'|'.join(names)})", get, "tensor",
+               tuple(names))
+
+
+def _mod(j, geo=None, i=None):
     names = ("shift_a", "scale_a", "gate_a", "shift_f", "scale_f", "gate_f")
+    if geo is not None and geo.layout is not None:
+        return _table(geo.layout, "mod", j, i)
     return E(f"modulation row {j} ({names[j]})", "mod", lambda m: m[:, j])
 
 
@@ -577,8 +737,8 @@ def block_stages(geo, wt, i):
     x += cross(norm3(x)); x += ffn(norm2(x)) * gate_f."""
     C, H = geo.C, geo.H
     kc = geo.kv_col * 2 * C
-    st = [_norm_stage("norm1", geo, X_IN, _mod(1), _mod(0))]
-    st += self_attention_stages(geo, wt, i, _act("norm1", geo), X_IN, EPI["GATE_RES"], gate=_mod(2), tok=True)
+    st = [_norm_stage("norm1", geo, X_IN, _mod(1, geo, i), _mod(0, geo, i))]
+    st += self_attention_stages(geo, wt, i, _act("norm1", geo), X_IN, EPI["GATE_RES"], gate=_mod(2, geo, i), tok=True)
     st.append(_norm_stage("norm3", geo, S("o"), w=wt.vec(i, "norm3.weight"), b=wt.vec(i, "norm3.bias")))
     st.append(_gemm_stage("cross_q", geo, _act("norm3", geo), wt.lin(i, ["cross_attn.q"]), wt.bias(i, ["cross_attn.q"]),
                           EPI["BF16"]))
@@ -601,11 +761,11 @@ def block_stages(geo, wt, i):
         att = "cross_q8"
     st.append(_gemm_stage("cross_o", geo, _act(att, geo), wt.lin(i, ["cross_attn.o"]), wt.bias(i, ["cross_attn.o"]),
                           EPI["GATE_RES"], out_src=S("o")))
-    st.append(_norm_stage("norm2", geo, S("cross_o"), _mod(4), _mod(3)))
+    st.append(_norm_stage("norm2", geo, S("cross_o"), _mod(4, geo, i), _mod(3, geo, i)))
     st.append(_gemm_stage("ffn0", geo, _act("norm2", geo), wt.lin(i, ["ffn.0"]), wt.bias(i, ["ffn.0"]),
                           EPI["GELU"] if geo.precision == "bf16" else EPI["GELU_FP8"]))
     st.append(_gemm_stage("ffn2", geo, _act("ffn0", geo), wt.lin(i, ["ffn.2"]), wt.bias(i, ["ffn.2"]), EPI["GATE_RES"],
-                          out_src=S("cross_o"), gate=_mod(5), tok=True))
+                          out_src=S("cross_o"), gate=_mod(5, geo, i), tok=True))
     return st
 
 
@@ -616,12 +776,13 @@ def cross_kv_stages(geo, wt, ids):
     n_img = 257 if geo.variant == "14b" else 0
     g = dict(epilogue=V(EPI["BF16"]), gate=NONE, tok_idx=NONE, n_split=V(0), a_split=V(0), shape=NONE, res=NONE)
     w, b = wt.kv(ids, False)
-    st = [Stage("ckv", "gemm", dict(a=E("context text rows", "ctx", lambda c: c[n_img:]), w=w, bias=b, **g),
-                {"": lambda a: a["out"]}, check_gemm)]
+    fwd = geo.layout is not None          # the context phase's outputs, else the context the seam's caller hands in
+    txt = S("text2") if fwd else E("context text rows", "ctx", lambda c: c[n_img:])
+    st = [Stage("ckv", "gemm", dict(a=txt, w=w, bias=b, **g), {"": lambda a: a["out"]}, check_gemm)]
     if n_img:
         w, b = wt.kv(ids, True)
-        st.append(Stage("ckv_img", "gemm", dict(a=E("context image rows", "ctx", lambda c: c[:n_img]), w=w, bias=b, **g),
-                        {"": lambda a: a["out"]}, check_gemm))
+        img = S("img_ln4") if fwd else E("context image rows", "ctx", lambda c: c[:n_img])
+        st.append(Stage("ckv_img", "gemm", dict(a=img, w=w, bias=b, **g), {"": lambda a: a["out"]}, check_gemm))
     for j, i in enumerate(ids):
         cols = (j * 2 * C, j * 2 * C + C)
         rr = dict(rope=NONE, head_dim=V(D), eps=V(EPS), pieces=NONE)
@@ -634,6 +795,122 @@ def cross_kv_stages(geo, wt, ids):
     return st
 
 
+def _gemm16(name, a, w, bias, epi):
+    """A bf16 GEMM outside the block (embedders, text and image MLPs): no gate, no split layout."""
+    ins = dict(a=a, w=w, bias=bias, epilogue=V(epi), gate=NONE, tok_idx=NONE, n_split=V(0), a_split=V(0), shape=NONE, res=NONE)
+    return Stage(name, "gemm", ins, {"": lambda x: x["out"]}, check_gemm)
+
+
+def _sd16(sd, name, dev, pad_k=1, pad_n=1):
+    """Weight `name` [N, ...] flattened to [N, K] bf16, K zero-padded to a multiple of pad_k (the 16-byte row pitch TMA needs)
+    and N to a multiple of pad_n; its bias f32, zero-padded alike."""
+    w = sd[name + ".weight"].flatten(1).to(device=dev, dtype=torch.bfloat16)
+    b = sd[name + ".bias"].to(device=dev, dtype=torch.float32)
+    N, K = w.shape
+    Np, Kp = -(-N // pad_n) * pad_n, -(-K // pad_k) * pad_k
+    wp = torch.zeros(Np, Kp, dtype=torch.bfloat16, device=dev)
+    wp[:N, :K] = w
+    bp = torch.zeros(Np, dtype=torch.float32, device=dev)
+    bp[:N] = b
+    lab = f"{name}" + (f" (K padded to {Kp})" if Kp != K else "") + (f" (N padded to {Np})" if Np != N else "")
+    return T(f"bf16 {lab}.weight", wp), T(f"{lab}.bias", bp)
+
+
+def _sd32(sd, name, dev, shape=None):
+    t = sd[name].to(device=dev, dtype=torch.float32)
+    return T(name, (t.reshape(shape) if shape else t).contiguous())
+
+
+def _patchify_stage(name, x, patch):
+    return Stage(name, "patchify", dict(x=x, ph=V(patch), pw=V(patch)), {"": lambda a: a["out"]}, check_patchify)
+
+
+def embed_stages(lay, sd, dev):
+    """One patchify + GEMM (EPI_F32 into the segment's rows of the stream) per segment in token order (model.py:599-729); the
+    deepest FramePack level runs patchify(4x4) + the patch_embedding_2x_f GEMM (N = in_dim padded to 32) in front, and its
+    embedder reads that GEMM's output as [in_dim, f, ceil(H/4), ceil(W/4)]. The grid path is one segment."""
+    cin = lay.x.shape[0]
+    st = []
+    for k, sg in enumerate(lay.segs):
+        fr = f"frames [{sg.f0}:{sg.f1}]"
+        if sg.pre_2x_f:
+            H, W = lay.x.shape[2:]
+            h2, w2, f = -(-H // 4), -(-W // 4), sg.f1 - sg.f0
+            st.append(_patchify_stage(f"embed[{k}].2x_f.patchify",
+                                      Src(f"x[:, {sg.f0}:{sg.f1}]", lambda ck, sg=sg: lay.x[:, sg.f0:sg.f1]), 4))
+            st.append(_gemm16(f"embed[{k}].2x_f", S(f"embed[{k}].2x_f.patchify"),
+                              *_sd16(sd, "patch_embedding_2x_f", dev, 8, 32), EPI["F32"]))
+            x = S(f"embed[{k}].2x_f", fn=lambda t, f=f, h2=h2, w2=w2: t[:, :cin].t().reshape(cin, f, h2, w2),
+                  what=f"[:, :{cin}] as [{cin}, {f}, {h2}, {w2}]")
+        else:
+            hh, ww = (sg.grid[1] * sg.patch, sg.grid[2] * sg.patch) if sg.crop else lay.x.shape[2:]
+            x = Src(f"x[:, {sg.f0}:{sg.f1}, :{hh}, :{ww}]", lambda ck, sg=sg, hh=hh, ww=ww: lay.x[:, sg.f0:sg.f1, :hh, :ww])
+        st.append(_patchify_stage(f"embed[{k}].patchify", x, sg.patch))
+        st.append(_gemm16(f"embed[{k}]", S(f"embed[{k}].patchify"), *_sd16(sd, sg.name, dev, 8), EPI["F32"]))
+    return st
+
+
+def time_stages(lay, sd, dev, C):
+    """Per chunk of at most 16 table rows (model.py:805-812, 296, 344): sinusoid(t) -> time_embedding.0 -> SiLU ->
+    time_embedding.2 = e -> SiLU -> time_projection.1 = e0; block table = blocks.*.modulation + e0, head table = e +
+    head.modulation."""
+    mods = T("blocks.*.modulation [layers, 6C]", torch.stack([sd[f"blocks.{i}.modulation"].reshape(-1) for i in range(lay.layers)])
+             .to(device=dev, dtype=torch.float32).contiguous())
+    st = []
+    for c, s0 in enumerate(range(0, len(lay.t_rows), T_CHUNK)):
+        rows = lay.t_rows[s0:s0 + T_CHUNK]
+        p = f"time[{c}]"
+        lin = lambda name, x, w, silu: Stage(  # noqa: E731
+            name, "linear_f32_small", dict(x=x, w=_sd32(sd, w + ".weight", dev), bias=_sd32(sd, w + ".bias", dev), silu_in=V(silu)),
+            {"": lambda a: a["ret"]}, check_lfs)
+        st.append(Stage(f"{p}.sinusoidal", "sinusoidal",
+                        dict(t=T(f"timesteps {rows}", torch.tensor(rows, dtype=torch.float32, device=dev)), dim=V(sd[
+                            "time_embedding.0.weight"].shape[1])), {"": lambda a: a["ret"]}, check_sin))
+        st.append(lin(f"{p}.emb0", S(f"{p}.sinusoidal"), "time_embedding.0", False))
+        st.append(lin(f"{p}.emb2", S(f"{p}.emb0"), "time_embedding.2", True))
+        st.append(lin(f"{p}.proj", S(f"{p}.emb2"), "time_projection.1", True))
+        st.append(Stage(f"{p}.mod", "bcast_add", dict(a=mods, b=S(f"{p}.proj")), {"": lambda a: a["ret"]}, check_bcast))
+        st.append(Stage(f"{p}.head", "bcast_add", dict(a=S(f"{p}.emb2"), b=_sd32(sd, "head.modulation", dev, (2, C))),
+                        {"": lambda a: a["ret"]}, check_bcast))
+    return st
+
+
+def context_stages(lay, sd, dev, variant, text_len):
+    """text_embedding on the context zero-padded to text_len rows: Linear, GELU(tanh), Linear (model.py:815-821); on 14B the
+    MLPProj of the CLIP features: LayerNorm (eps 1e-5), Linear, GELU(erf), Linear, LayerNorm (wan/modules/model.py:529-541)."""
+    ctx = lay.context.to(device=dev, dtype=torch.bfloat16)
+    pad = torch.cat([ctx, ctx.new_zeros(text_len - ctx.shape[0], ctx.shape[1])])
+    st = [_gemm16("text0", T(f"context ({ctx.shape[0]} rows) zero-padded to {text_len} rows", pad),
+                  *_sd16(sd, "text_embedding.0", dev), EPI["GELU"]),
+          _gemm16("text2", S("text0"), *_sd16(sd, "text_embedding.2", dev), EPI["BF16"])]
+    if variant == "14b":
+        def ln(name, x, key):
+            return Stage(name, "ln_modulate", dict(x=x, scale=NONE, shift=NONE, tok_idx=NONE, weight=_sd32(sd, key + ".weight", dev),
+                                                   bias=_sd32(sd, key + ".bias", dev), eps=V(IMG_EPS)),
+                         {"": lambda a: a["out"]}, check_ln)
+        st.append(ln("img_ln0", T("clip_fea rows (f32)", lay.clip.to(device=dev, dtype=torch.float32).contiguous()),
+                     "img_emb.proj.0"))
+        st.append(_gemm16("img_fc1", S("img_ln0"), *_sd16(sd, "img_emb.proj.1", dev), EPI["GELU_ERF"]))
+        st.append(_gemm16("img_fc3", S("img_fc1"), *_sd16(sd, "img_emb.proj.3", dev), EPI["F32"]))
+        st.append(ln("img_ln4", S("img_fc3"), "img_emb.proj.4"))
+    return st
+
+
+def head_stages(geo, sd, dev):
+    """Head.forward (model.py:336-348; wan/modules/model.py:516-526): LayerNorm * (1 + head row 1) + head row 0 of every token's
+    timestep (built from e, not e0), head.head into f32, then unpatchify of rows [L_hist:] over the new frames' grid
+    (model.py:867-890). The input is the last block's final GATE_RES output."""
+    lay = geo.layout
+    f, h, w = lay.grid
+    return [Stage("head_ln", "ln_modulate", dict(x=S("ffn2"), scale=_table(lay, "head", 1), shift=_table(lay, "head", 0),
+                                                 tok_idx=_tok(geo), weight=NONE, bias=NONE, eps=V(EPS)),
+                  {"": lambda a: a["out"]}, check_ln),
+            Stage("head_lin", "linear_f32", dict(x=S("head_ln"), w=_sd32(sd, "head.head.weight", dev),
+                                                 bias=_sd32(sd, "head.head.bias", dev)), {"": lambda a: a["out"]}, check_lin32),
+            Stage("unpatchify", "unpatchify", dict(y=S("head_lin", rows=(lay.L_hist, None)), F=V(f), Hp=V(h), Wp=V(w), ph=V(2),
+                                                   pw=V(2)), {}, check_unpatchify)]
+
+
 # ------------------------------------------------------------------------------------------------------------
 # running a cell
 # ------------------------------------------------------------------------------------------------------------
@@ -643,11 +920,8 @@ def rope_rows(freqs):
 
 
 def install(mp, dit_module, eng, sd, geo, i, tag, kv_ids, seam="block", att_plan=None, target_call=None):
-    """Put a checker for block i (and the cross K|V launches of blocks kv_ids, unless seam == 'self_attention') between `eng` and
-    its ops module. The engine then runs unchanged: _context / _time_tables hand the checker the embedded context and the
-    modulation table, _cross_kv is the cross K|V region, the `target_call`-th _block_body call (default: the one for block i)
-    the block region. Returns the checker; ck.env takes 'x_in' (and for seams 'ctx', 'mod') from the caller where the engine
-    does not produce them."""
+    """A checker for one seam call: block_forward (seam 'block': the one-block cross K|V launches of kv_ids, then block i) or
+    self_attention_forward. The caller hands in ck.env's 'x_in', 'ctx' and 'mod'."""
     ck = Checker(dit_module.ops, tag, att_plan)
     dev = geo.rope.device
     wt = Weights(sd, geo.precision, dev)
@@ -660,20 +934,8 @@ def install(mp, dit_module, eng, sd, geo, i, tag, kv_ids, seam="block", att_plan
         ck.add_phase("cross_kv", cross_kv_stages(geo, wt, kv_ids))
         ck.add_phase("block", block_stages(geo, wt, i))
     mp.setattr(dit_module, "ops", ck.proxy)
-    real_context, real_tables, real_kv = eng._context, eng._time_tables, eng._cross_kv
-    real_body, real_sa = eng._block_body, eng.self_attention_forward
+    real_kv, real_body, real_sa = eng._cross_kv, eng._block_body, eng.self_attention_forward
     calls = {"body": 0}
-
-    def context(*a, **k):
-        out = real_context(*a, **k)
-        ck.env["ctx"] = out.clone()
-        return out
-
-    def tables(*a, **k):
-        e, mod, head = real_tables(*a, **k)
-        ck.env["mod_table"] = mod.clone()
-        ck.env["mod"] = ck.env["mod_table"][i]
-        return e, mod, head
 
     def cross_kv(*a, **k):
         with ck.region("cross_kv"):
@@ -684,16 +946,12 @@ def install(mp, dit_module, eng, sd, geo, i, tag, kv_ids, seam="block", att_plan
         calls["body"] += 1
         if n != (i if target_call is None else target_call):
             return real_body(j, xs, *a, **k)
-        if "x_in" not in ck.env:
-            ck.env["x_in"] = ck.stream.clone()
         with ck.region("block"):
             return real_body(j, xs, *a, **k)
 
     def self_attention(*a, **k):
         with ck.region("self_attention"):
             return real_sa(*a, **k)
-    mp.setattr(eng, "_context", context)
-    mp.setattr(eng, "_time_tables", tables)
     if seam == "self_attention":
         mp.setattr(eng, "self_attention_forward", self_attention)
     else:
@@ -702,56 +960,182 @@ def install(mp, dit_module, eng, sd, geo, i, tag, kv_ids, seam="block", att_plan
     return ck
 
 
-def check_modulation_rows(ck, sd, cfg, i, t_rows):
-    """Row u of the engine's modulation table for block i is blocks.i.modulation + time_projection(t_rows[u]) (the reference's
-    e0, model.py:805-812, recomputed by the oracle): pins which timestep each row stands for, so that a token index pointing at
-    a row is a statement about the token's timestep."""
-    orc = WanOracle(sd, **synth.oracle_kwargs(cfg))
-    _, e0 = orc.time_embed(torch.tensor(t_rows, dtype=torch.float32))
-    want = sd[f"blocks.{i}.modulation"].reshape(1, 6, -1).double() + e0.double().view(len(t_rows), 6, -1)
-    got = ck.env["mod_table"][i].double().cpu()
-    assert got.shape == want.shape, f"{ck.tag}: modulation table rows {tuple(got.shape)}, want {tuple(want.shape)}"
-    err = float((got - want).abs().max() / want.abs().max())
-    assert err < 1e-3, f"{ck.tag}: modulation row order: rows differ from the timesteps {t_rows} by {err:.2e}"
+PHASES = ("embed", "time", "context", "cross_kv", "block", "head")
+
+
+def check_stream(ck, lay, xs, tok):
+    """The residual stream and the token index the first block receives: rows [row0, row0 + n) of every segment equal to that
+    segment's embed GEMM output, the rows past n_real exact zeros; tok_idx the geometry's (every token -> its timestep's row)."""
+    what = "block 0 input"
+    if tuple(xs.shape) != (lay.L, xs.shape[1]):
+        raise AssertionError(f"{ck.tag}: stage '{what}' operand 'xs' has {xs.shape[0]} rows, the spec's stream {lay.L}")
+    for k, sg in enumerate(lay.segs):
+        _same(ck.tag, what, "xs", xs[sg.row0:sg.row0 + sg.n], ck.snap[f"embed[{k}]"][""],
+              Src(f"embed[{k}] (the {sg.name} GEMM) at rows [{sg.row0}:{sg.row0 + sg.n}]", None))
+    _same(ck.tag, what, "xs", xs[lay.n_real:], torch.zeros_like(xs[lay.n_real:]),
+          Src(f"zero padding tokens at rows [{lay.n_real}:{lay.L}]", None))
+    _same(ck.tag, what, "tok_idx", tok, ck.geo.tok, T("each token's timestep row", ck.geo.tok) if ck.geo.tok is not None else NONE)
+    ck.unpin()
+
+
+def install_forward(mp, dit_module, eng, sd, geo, i, tag, att_plan=None):
+    """Put a checker for the whole forward between `eng` and its ops module: every launch from the token stream to unpatchify
+    is the spec's, except those of the blocks other than i (which pass through; block i must be the last, so that the head
+    reads its output). The phases open as the engine reaches them: embed at _token_stream, time at the first _time_tables,
+    context at _context, cross_kv around _cross_kv, block around the i-th _block_body, head after the last; the forward must
+    have entered all six in that order."""
+    lay = geo.layout
+    assert i == lay.layers - 1, "the head reads the checked block's output: check the last block"
+    ck = Checker(dit_module.ops, tag, att_plan)
+    ck.geo = geo
+    dev = geo.rope.device
+    wt = Weights(sd, geo.precision, dev)
+    ck.add_phase("embed", embed_stages(lay, sd, dev))
+    ck.add_phase("time", time_stages(lay, sd, dev, geo.C))
+    ck.add_phase("context", context_stages(lay, sd, dev, geo.variant, eng.text_len))
+    ck.add_phase("cross_kv", cross_kv_stages(geo, wt, list(range(lay.layers))))
+    ck.add_phase("block", block_stages(geo, wt, i))
+    ck.add_phase("head", head_stages(geo, sd, dev))
+    ck.pinned = {f"embed[{k}]" for k in range(len(lay.segs))}
+    mp.setattr(dit_module, "ops", ck.proxy)
+    real = {n: getattr(eng, n) for n in ("_token_stream", "_time_tables", "_context", "_cross_kv", "_block_body",
+                                         "_forward_eager")}
+    calls = {"body": 0}
+
+    def token_stream(*a, **k):
+        out = real["_token_stream"](*a, **k)
+        ck.enter("embed")
+        return out
+
+    def tables(*a, **k):
+        if ck.phase != "time":
+            ck.enter("time")
+        return real["_time_tables"](*a, **k)
+
+    def context(*a, **k):
+        ck.enter("context")
+        return real["_context"](*a, **k)
+
+    def cross_kv(*a, **k):
+        ck.enter("cross_kv")
+        out = real["_cross_kv"](*a, **k)
+        ck.leave()
+        return out
+
+    def body(j, xs, m, tok, *a, **k):
+        n = calls["body"]
+        calls["body"] += 1
+        if n == 0:
+            ck.leave()
+            check_stream(ck, lay, xs, tok)
+        if n == i:
+            ck.env["x_in"] = ck.stream.clone() if n else xs.clone()
+            with ck.region("block"):
+                out = real["_block_body"](j, xs, m, tok, *a, **k)
+        else:
+            out = real["_block_body"](j, xs, m, tok, *a, **k)
+        if n == lay.layers - 1:
+            ck.enter("head")
+        return out
+
+    def forward(*a, **k):
+        out = real["_forward_eager"](*a, **k)
+        ck.leave()
+        if tuple(ck.entered) != PHASES:
+            raise AssertionError(f"{ck.tag}: the forward ran the phases {ck.entered}, the spec's are {list(PHASES)}")
+        return out
+    for n, f in (("_token_stream", token_stream), ("_time_tables", tables), ("_context", context), ("_cross_kv", cross_kv),
+                 ("_block_body", body), ("_forward_eager", forward)):
+        mp.setattr(eng, n, f)
+    return ck
 
 
 # ------------------------------------------------------------------------------------------------------------
 # paths: the inputs of one forward and the geometry the spec derives from them (oracle.wan_dit, not dit.py)
 # ------------------------------------------------------------------------------------------------------------
-def path_inputs(cfg, path, frames, H, W, lfz=None, pad=0, seed=0):
-    """Forward arguments of a path: '5b_grid' (scalar t, seq_len = L_grid + pad: padding rows are keys on the 5B tree),
-    '5b_framepack' (history t[0], new frames t[-1]), '14b_framepack' (image branch), '14b_grid_padded' (seq_len = L_grid + pad:
-    padding rows are not keys)."""
-    inp = synth.make_inputs(cfg, seed, frames, H, W, 24)
+def path_inputs(cfg, path, frames, H, W, lfz=None, pad=0, seed=0, ctx_len=24, t=None):
+    """Forward arguments of a path: '5b_grid' (scalar t, seq_len = L_grid + pad: padding rows are keys on the 5B tree; `t` a
+    per-frame list gives a per-token t over seq_len = L_grid), '5b_framepack' (history t[0], new frames t[-1]), '14b_framepack'
+    (image branch), '14b_grid_padded' (seq_len = L_grid + pad: padding rows are not keys)."""
+    inp = synth.make_inputs(cfg, seed, frames, H, W, ctx_len)
     packed = "framepack" in path
     L_grid = frames * (H // 2) * (W // 2)
-    args = dict(x=inp["x"], t=torch.tensor([700.0]) if not (packed and cfg["variant"] == "5b") else torch.tensor([0.0, 900.0]),
-                context=inp["context"], seq_len=L_grid + pad, packed=packed, latent_frame_zero=lfz)
+    if t is not None:
+        assert not packed and pad == 0 and len(t) == frames
+        tt = torch.tensor(t, dtype=torch.float32).repeat_interleave(L_grid // frames)
+    else:
+        tt = torch.tensor([700.0]) if not (packed and cfg["variant"] == "5b") else torch.tensor([0.0, 900.0])
+    args = dict(x=inp["x"], t=tt, context=inp["context"], seq_len=L_grid + pad, packed=packed, latent_frame_zero=lfz)
     if cfg["variant"] == "14b":
         args.update(y=inp["y"], clip_fea=inp["clip_fea"])
     return args
 
 
-def path_geometry(cfg, sd, precision, args, dev):
-    """Geometry of a forward from the oracle's own token layout: k_len, RoPE rows, token index, modulation timesteps."""
+def warm_inputs(cfg, path, frames, H, W, lfz=None, pad=0, seed=0, t=None):
+    """What an earlier forward on the same engine leaves in the reused workspaces: a prompt of text_len rows and, on a padded
+    grid, the largest grid that fits the same seq_len (so the padding rows of the checked run hold non-zero tokens)."""
+    if "framepack" in path or pad == 0:
+        return path_inputs(cfg, path, frames, H, W, lfz, pad, seed + 1, ctx_len=cfg["text_len"], t=t)
+    seq_len = frames * (H // 2) * (W // 2) + pad
+    best = max(((f * h * w, f, h, w) for f in range(1, 2 * frames + 1) for h in range(H // 2, H + 1)
+                for w in range(W // 2, W + 1) if f * h * w <= seq_len), key=lambda c: c[0])
+    _, f, h, w = best
+    args = path_inputs(cfg, path, f, 2 * h, 2 * w, lfz, 0, seed + 1, ctx_len=cfg["text_len"])
+    args["seq_len"] = seq_len
+    return args
+
+
+def path_geometry(cfg, sd, precision, args, dev, layers=None):
+    """Geometry of a forward from the reference's own token layout (WanOracle._segments, the convpadd and plain-Conv3d shapes,
+    grid_freqs): the segments and their rows, k_len, RoPE rows, timestep rows and each token's row."""
     orc = WanOracle(sd, **synth.oracle_kwargs(cfg))
     x = args["x"] if args.get("y") is None else torch.cat([args["x"], args["y"]], 0)
     five = cfg["variant"] == "5b"
+    _, Ft, Hh, Ww = x.shape
+    segs, freqs, row = [], [], 0
+
+    def add(f0, f1, name, pre, padm, fz):
+        nonlocal row
+        p = sd[name + ".weight"].shape[-1]
+        h, w = (-(-Hh // 4), -(-Ww // 4)) if pre else (Hh, Ww)
+        g = (f1 - f0, -(-h // p), -(-w // p)) if padm else (f1 - f0, h // p, w // p)
+        segs.append(Segment(f0, f1, name, p, pre, not padm, g, row))
+        freqs.append(grid_freqs(orc.tables, *g, fz))
+        row += segs[-1].n
+        return fz + g[0]
     if args["packed"]:
         lfz = args["latent_frame_zero"] or (8 if five else 9)
-        tok, freqs, n_hist, _ = orc.pack(x.float(), lfz)
-        L, k_len = tok.shape[1], tok.shape[1]
-        tok_idx = torch.cat([torch.zeros(n_hist), torch.ones(L - n_hist)]).to(torch.int32) if five else None
-        t_rows = [float(args["t"][0]), float(args["t"][-1])] if five else [float(args["t"][0])]
+        hist = Ft - lfz
+        fz = 0
+        for sl, name, padm, pre in orc._segments(hist, Ft - (lfz if five else 9)):
+            fr = range(hist)[sl]
+            fz = add(fr.start, fr.stop, name, pre, padm, fz)
+        L_hist = row
+        add(hist, Ft, "patch_embedding", False, 0, fz)
+        L = n_real = k_len = row
     else:
-        f, h, w = x.shape[1], x.shape[2] // 2, x.shape[3] // 2
-        freqs = grid_freqs(orc.tables, f, h, w)
-        L = args["seq_len"]
-        k_len = L if five else f * h * w
-        tok_idx, t_rows = None, [float(args["t"][0])]
-    geo = Geometry(cfg["variant"], precision, cfg["dim"], cfg["num_heads"], k_len, rope_rows(freqs).to(dev),
-                   None if tok_idx is None else tok_idx.to(dev))
-    return geo, L, t_rows
+        add(0, Ft, "patch_embedding", False, 0, 0)
+        L_hist, n_real, L = 0, row, args["seq_len"]
+        k_len = L if five else n_real
+    t = args["t"].flatten().float()
+    tok = None
+    if not five:
+        t_rows = [float(t[0])]
+    elif args["packed"]:
+        t_rows = [float(t[0]), float(t[-1])]
+        tok = torch.cat([torch.zeros(L_hist), torch.ones(L - L_hist)]).to(torch.int32)
+    elif t.numel() == 1:
+        t_rows = [float(t[0])]
+    else:
+        vals = sorted(set(t.tolist()))
+        t_rows = vals
+        tok = torch.searchsorted(torch.tensor(vals, dtype=torch.float32), t).to(torch.int32)
+    clip = args.get("clip_fea")
+    lay = Layout(x.float().to(dev), segs, L, n_real, L_hist, segs[-1].grid, t_rows, args["context"],
+                 None if clip is None else clip.reshape(-1, clip.shape[-1]), layers or cfg["num_layers"])
+    geo = Geometry(cfg["variant"], precision, cfg["dim"], cfg["num_heads"], k_len, rope_rows(torch.cat(freqs)).to(dev),
+                   None if tok is None else tok.to(dev), layout=lay)
+    return geo
 
 
 def engine_forward(eng, args):
@@ -762,19 +1146,21 @@ def engine_forward(eng, args):
 def oracle_forward(orc, cfg, args):
     kw = dict(seq_len=args["seq_len"], latent_frame_zero=args["latent_frame_zero"])
     if cfg["variant"] == "5b":
-        return orc.forward([args["x"]], args["t"], [args["context"]], flag=args["packed"], **kw)
+        t = args["t"] if args["packed"] or args["t"].numel() == 1 else args["t"].view(1, -1)   # per-token t: [B, seq_len]
+        return orc.forward([args["x"]], t, [args["context"]], flag=args["packed"], **kw)
     return orc.forward([args["x"]], args["t"], [args["context"]], y=[args["y"]], clip_fea=args["clip_fea"],
                        rand_num_img=0.5 if args["packed"] else 0.1, **kw)
 
 
-def run_path(mp, dit_module, eng, sd, cfg, precision, args, i, tag, att_plan=None):
-    """The engine's forward with block i and the all-layer cross K|V launches checked. Returns the checker."""
-    dev = eng.device
-    geo, L, t_rows = path_geometry(cfg, sd, precision, args, dev)
+def run_path(mp, dit_module, eng, sd, cfg, precision, args, i, tag, att_plan=None, warm=None):
+    """The engine's forward checked launch by launch with block i (the last) in full; `warm`: the arguments of an unchecked
+    forward run first on the same engine, whose leftovers the checked run must not read. Returns the checker."""
+    if warm is not None:
+        engine_forward(eng, warm)
+    geo = path_geometry(cfg, sd, precision, args, eng.device, eng.layers)
     geo.kv_col = i
-    ck = install(mp, dit_module, eng, sd, geo, i, tag, list(range(eng.layers)), att_plan=att_plan)
+    ck = install_forward(mp, dit_module, eng, sd, geo, i, tag, att_plan=att_plan)
     engine_forward(eng, args)
-    check_modulation_rows(ck, sd, cfg, i, t_rows)
     return ck
 
 

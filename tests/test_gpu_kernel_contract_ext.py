@@ -728,6 +728,36 @@ def test_blend_is_the_reference_expression(dev, dim, ext):
 # ------------------------------------------------------------------------------------------------------------
 # fp32 DiT ops
 # ------------------------------------------------------------------------------------------------------------
+def sinusoidal_ref(t, dim):
+    """(ref, bound) of yb_sinusoidal on f32 timesteps t [U] (test_sinusoidal_per_element derives the bound)."""
+    half = dim // 2
+    s = torch.outer(t.double(), torch.pow(10000.0, -torch.arange(half, device=t.device, dtype=torch.float64) / half))
+    ref = torch.cat([s.cos(), s.sin()], 1)
+    e = 2.0 ** -50 * (1 + t.double().abs())[:, None]
+    return ref, U32 * (ref.abs() + e) + e
+
+
+def linear_f32_small_ref(x, w, bias, silu):
+    """(ref, bound) of yb_linear_f32_small on x [M, K], w [N, K] (test_linear_f32_small_per_element derives the bound)."""
+    K, N = x.shape[1], w.shape[0]
+    a = x.double()
+    if silu:
+        a = a * torch.sigmoid(a)
+    ref = a @ w.double().t()
+    bd = bias.double() if bias is not None else torch.zeros(N, dtype=torch.float64, device=x.device)
+    aw = a.abs() @ w.double().abs().t()
+    return ref + bd, (K / 32 + 6 + (6 if silu else 0)) * U32 * aw + U32 * (ref + bd).abs()
+
+
+def linear_f32_ref(x, w, bias):
+    """(ref, bound) of yb_linear_f32 on x [M, K], w [N, K] (test_linear_f32_per_element derives the bound)."""
+    K = x.shape[1]
+    ref = x.double() @ w.double().t()
+    if bias is not None:
+        ref = ref + bias.double()
+    return ref, K * U32 * (x.double().abs() @ w.double().abs().t()) + U32 * ref.abs()
+
+
 def test_sinusoidal_per_element(dev):
     """yb_sinusoidal: t = 0, integers up to 1000 and non-integer sampler timesteps; dim 256. The kernel evaluates
     pos * 10000^(-i/half), cos and sin in fp64 (each within a few fp64 ulps: the argument |a| <= |t| is off by <= 4*2^-53*|t|,
@@ -735,15 +765,13 @@ def test_sinusoidal_per_element(dev):
     from yume_b200 import _lib, ops
     t = torch.tensor([0.0, 1.0, 2.0, 17.0, 250.0, 999.0, 1000.0, 0.5, 3.25, 937.8125, 12.3456, 999.999, 0.001],
                      device=dev, dtype=torch.float32)
-    dim, half = 256, 128
+    dim = 256
     out = guarded((t.numel(), dim), torch.float32, (2, 0))
     assert _lib.load().yb_sinusoidal(t.data_ptr(), out.view.data_ptr(), t.numel(), dim, ops._stream()) == 0
     torch.cuda.synchronize()
     out.check("sinusoidal")
-    s = torch.outer(t.double(), torch.pow(10000.0, -torch.arange(half, device=dev, dtype=torch.float64) / half))
-    ref = torch.cat([s.cos(), s.sin()], 1)
-    e = 2.0 ** -50 * (1 + t.double().abs())[:, None]
-    assert_within(out.view, ref, U32 * (ref.abs() + e) + e, "sinusoidal dim256", "sinusoidal")
+    ref, bound = sinusoidal_ref(t, dim)
+    assert_within(out.view, ref, bound, "sinusoidal dim256", "sinusoidal")
 
 
 @pytest.mark.parametrize("silu,with_bias", [(False, True), (True, True), (True, False)])
@@ -765,14 +793,8 @@ def test_linear_f32_small_per_element(dev, K, N, M, silu, with_bias):
     torch.cuda.synchronize()
     tag = f"linear_f32_small M{M} N{N} K{K} silu{int(silu)} bias{int(with_bias)}"
     out.check(tag)
-    a = x.double()
-    if silu:
-        a = a * torch.sigmoid(a)
-    ref = a @ w.double().t()
-    bd = bias.double() if with_bias else torch.zeros(N, dtype=torch.float64, device=dev)
-    aw = a.abs() @ w.double().abs().t()
-    bound = (K / 32 + 6 + (6 if silu else 0)) * U32 * aw + U32 * (ref + bd).abs()
-    assert_within(out.view, ref + bd, bound, tag, "linear_f32_small")
+    ref, bound = linear_f32_small_ref(x, w, bias, silu)
+    assert_within(out.view, ref, bound, tag, "linear_f32_small")
 
 
 @pytest.mark.parametrize("N", [64, 100, 192])
@@ -792,8 +814,7 @@ def test_linear_f32_per_element(dev, M, K, N):
     torch.cuda.synchronize()
     tag = f"linear_f32 M{M} K{K} N{N}"
     out.check(tag)
-    ref = x.double() @ w.double().t() + bias.double()
-    bound = K * U32 * (x.double().abs() @ w.double().abs().t()) + U32 * ref.abs()
+    ref, bound = linear_f32_ref(x, w, bias)
     assert_within(out.view, ref, bound, tag, "linear_f32")
 
 

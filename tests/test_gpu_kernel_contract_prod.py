@@ -380,6 +380,9 @@ def gemm_epilogue_ref(epi, acc, Fb, bias=None, res=None, x0=None, gate=None):
     if epi == EPI["GELU"]:
         ref = F.gelu(accb, approximate="tanh")
         return ref, bf16_out_bound(ref, 1.13 * f32 + 2.0 ** -12 * accb.abs() + 4 * U32 * accb.abs())
+    if epi == EPI["GELU_ERF"]:
+        ref = F.gelu(accb)
+        return ref, bf16_out_bound(ref, 1.13 * f32 + 2.0 ** -20 * accb.abs() + 4 * U32 * accb.abs())
     if epi == EPI["F32"]:
         return accb, f32
     if epi == EPI["RES_BF16"]:
