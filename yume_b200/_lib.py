@@ -151,6 +151,14 @@ FP8_ATTN_SIGNATURES = {
     "yb_attention_fp8": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, _vp, _ll, _i, _i, _i, _f, _i, _vp, _ll, _vp]),
 }
 
+# every symbol include/yume_b200_fp8_sp.h declares (precision="fp8" / "fp8_attn" under Ulysses sequence parallelism)
+FP8_SP_SIGNATURES = {
+    "yb_quant_rows_fp8_split": (_i, [_vp, _ll, _i, _ll, _vp, _ll, _vp, _ll, _i, _i, _vp]),
+    "yb_attention_fp8_sp": (_i, [_vp, _ll, _vp, _ll, _vp, _ll, _vp, _vp, C.POINTER(C.c_void_p), _ll, _i, _i, _i, _f, _i, _i, _i,
+                                 _i, _vp, _ll, _vp]),
+    "yb_sp_pack_qkv": (_i, [_vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _f, _vp, _i, _i, _vp]),
+}
+
 # every symbol include/yume_b200_fp8_vae.h declares (the e4m3 convs of Wan22VaeDecoder(precision="fp8"))
 class Conv3dFp8Args(C.Structure):
     """Mirror of `struct yb_conv3d_fp8_args` (include/yume_b200_fp8_vae.h)."""
@@ -194,7 +202,8 @@ def load():
         raise YumeB200Error(f"{_LIB_PATH} has ABI version {lib.yb_abi_version()}, this binding expects {ABI_VERSION}: rebuild it "
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
-                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES, **RESUME_SIGNATURES}.items():
+                              **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES, **RESUME_SIGNATURES,
+                              **FP8_SP_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

@@ -20,7 +20,8 @@ SOURCES = ["gemm.cu", "attention.cu", "elementwise.cu", "vae_elementwise.cu", "p
 HEADERS = ["yb_ptx.cuh", "yb_host.h", "../../include/yume_b200.h", "../../include/yume_b200_clip.h",
            "../../include/yume_b200_t5.h", "../../include/yume_b200_stream.h",
            "../../include/yume_b200_fp8.h", "../../include/yume_b200_fp8_attn.h",
-           "../../include/yume_b200_fp8_vae.h", "../../include/yume_b200_vae_resume.h"]
+           "../../include/yume_b200_fp8_vae.h", "../../include/yume_b200_vae_resume.h",
+           "../../include/yume_b200_fp8_sp.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

@@ -440,12 +440,17 @@ static int launch_attention(const CUtensorMap& tmQ, const CUtensorMap& tmK, cons
 
 // the combine for another attention kernel that writes its KV-segment partials in this layout (attention_fp8.cu)
 int attention_combine_launch(void* out, long long ldo, int Lq, int nq, int full_units, int ns, int tail, float* ws_o,
-                             float* ws_ml, cudaStream_t stream) {
+                             float* ws_ml, cudaStream_t stream, void* const* out_peers, int world, int rank, int Lp) {
   AttParams p = {};
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ldo = ldo;
   p.Lq = Lq;
-  p.sp_world = 1;
+  p.sp_world = out_peers ? world : 1;
+  if (out_peers) {
+    for (int i = 0; i < 8; ++i) p.out_peers[i] = i < world ? static_cast<__nv_bfloat16*>(out_peers[i]) : nullptr;
+    p.sp_rank = rank;
+    p.sp_Lp = Lp;
+  }
   p.nq = nq;
   p.full_units = full_units;
   p.ns = ns;

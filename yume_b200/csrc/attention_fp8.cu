@@ -30,6 +30,7 @@
 #include "yb_host.h"
 #include "../../include/yume_b200_fp8.h"
 #include "../../include/yume_b200_fp8_attn.h"
+#include "../../include/yume_b200_fp8_sp.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -78,10 +79,18 @@ __device__ __forceinline__ int a8_row_a() {
   return static_cast<int>((t >> 7) - 1) * 64 + static_cast<int>((t >> 5) & 3) * 16 + static_cast<int>((t & 31) >> 2);
 }
 
-__global__ void __launch_bounds__(A8_THREADS, 1)
-attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmSQ,
-                     const __grid_constant__ CUtensorMap tmSK, const Att8Params p) {
+// Ulysses (yb_attention_fp8_sp): output row g belongs to rank g / Lp and is stored into row rank * Lp + g % Lp of that rank's
+// [P(src), Lp, heads_local * 128] receive buffer over NVLink, as attention.cu's AttParams.out_peers
+struct Att8Peers {
+  __nv_bfloat16* out[8];
+  int world, rank, Lp;
+};
+
+// the kernel body; SP selects the epilogue's store address (attention_fp8_kernel / attention_fp8_sp_kernel), nothing else
+template <bool SP>
+__device__ __forceinline__ void attention_fp8_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
+                                                   const CUtensorMap& tmSQ, const CUtensorMap& tmSK, const Att8Params& p,
+                                                   const Att8Peers* sp) {
   constexpr int NS = A8_NS;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -323,7 +332,13 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
         uint32_t ln;
         asm volatile("mov.u32 %0, %%laneid;" : "=r"(ln));
         const int col0 = head * 128 + 2 * static_cast<int>(ln & 3);
-        __nv_bfloat16* orow = p.out + static_cast<long long>(q_row) * p.ldo + col0;
+        __nv_bfloat16* orow;
+        if constexpr (SP) {
+          const int owner = q_row / sp->Lp;   // < world: Lq == world * Lp
+          orow = sp->out[owner] + (static_cast<long long>(sp->rank) * sp->Lp + (q_row - owner * sp->Lp)) * p.ldo + col0;
+        } else {
+          orow = p.out + static_cast<long long>(q_row) * p.ldo + col0;
+        }
         const float inv = 1.0f / l;
 #pragma unroll
         for (int g = 0; g < 16; ++g)
@@ -331,6 +346,20 @@ attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_const
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(A8_THREADS, 1)
+attention_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                     const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmSQ,
+                     const __grid_constant__ CUtensorMap tmSK, const Att8Params p) {
+  attention_fp8_body<false>(tmQ, tmK, tmV, tmSQ, tmSK, p, nullptr);
+}
+
+__global__ void __launch_bounds__(A8_THREADS, 1)
+attention_fp8_sp_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
+                        const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmSQ,
+                        const __grid_constant__ CUtensorMap tmSK, const Att8Params p, const __grid_constant__ Att8Peers sp) {
+  attention_fp8_body<true>(tmQ, tmK, tmV, tmSQ, tmSK, p, &sp);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -409,10 +438,12 @@ extern "C" int yb_quant_vt_fp8(const void* v, long long ldv, void* vt8, void* v_
   return check_launch("quant_vt_fp8");
 }
 
-extern "C" int yb_attention_fp8(const void* q8, long long ldq, const void* k8, long long ldk, const void* qk_scale, long long lds,
+namespace yb {
+
+// yb_attention_fp8 and yb_attention_fp8_sp: sp == nullptr stores rows into `out`, otherwise into the owners' receive buffers
+static int launch_attention_fp8(const void* q8, long long ldq, const void* k8, long long ldk, const void* qk_scale, long long lds,
                                 const void* vt8, const void* v_scale, void* out, long long ldo, int Lq, int Lk, int heads,
-                                float scale, int flags, void* ws, long long ws_bytes, void* stream_) {
-  using namespace yb;
+                                float scale, int flags, void* ws, long long ws_bytes, const Att8Peers* sp, void* stream_) {
   if (!q8 || !k8 || !qk_scale || !vt8 || !v_scale || !out) return YB_ERR_ARG;
   if (Lq <= 0 || Lk <= 0 || heads <= 0 || lds < Lq || lds < Lk) return YB_ERR_ARG;
   if (flags & ~(7 << YB_ATT_SPLIT_SHIFT)) return YB_ERR_ARG;   // no accumulate, P-in-smem or emulation forms
@@ -462,10 +493,50 @@ extern "C" int yb_attention_fp8(const void* q8, long long ldq, const void* k8, l
     }
   }
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  static bool attr_set[kMaxDevices] = {false};
-  if (int e = ensure_dynamic_smem(attention_fp8_kernel, A8_SMEM_BYTES, attr_set, "attention_fp8")) return e;
-  attention_fp8_kernel<<<p.full_units + tail * p.ns, A8_THREADS, A8_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmSQ, tmSK, p);
-  rc = check_launch("attention_fp8");
+  const int grid = p.full_units + tail * p.ns;
+  if (sp) {
+    static bool attr_set[kMaxDevices] = {false};
+    if (int e = ensure_dynamic_smem(attention_fp8_sp_kernel, A8_SMEM_BYTES, attr_set, "attention_fp8_sp")) return e;
+    attention_fp8_sp_kernel<<<grid, A8_THREADS, A8_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmSQ, tmSK, p, *sp);
+    rc = check_launch("attention_fp8_sp");
+  } else {
+    static bool attr_set[kMaxDevices] = {false};
+    if (int e = ensure_dynamic_smem(attention_fp8_kernel, A8_SMEM_BYTES, attr_set, "attention_fp8")) return e;
+    attention_fp8_kernel<<<grid, A8_THREADS, A8_SMEM_BYTES, stream>>>(tmQ, tmK, tmV, tmSQ, tmSK, p);
+    rc = check_launch("attention_fp8");
+  }
   if (rc || tail == 0) return rc;
+  if (sp)
+    return attention_combine_launch(p.out, p.ldo, Lq, p.nq, p.full_units, p.ns, tail, p.ws_o, p.ws_ml, stream,
+                                    reinterpret_cast<void* const*>(sp->out), sp->world, sp->rank, sp->Lp);
   return attention_combine_launch(p.out, p.ldo, Lq, p.nq, p.full_units, p.ns, tail, p.ws_o, p.ws_ml, stream);
+}
+
+}  // namespace yb
+
+extern "C" int yb_attention_fp8(const void* q8, long long ldq, const void* k8, long long ldk, const void* qk_scale, long long lds,
+                                const void* vt8, const void* v_scale, void* out, long long ldo, int Lq, int Lk, int heads,
+                                float scale, int flags, void* ws, long long ws_bytes, void* stream_) {
+  return yb::launch_attention_fp8(q8, ldq, k8, ldk, qk_scale, lds, vt8, v_scale, out, ldo, Lq, Lk, heads, scale, flags, ws,
+                                  ws_bytes, nullptr, stream_);
+}
+
+extern "C" int yb_attention_fp8_sp(const void* q8, long long ldq, const void* k8, long long ldk, const void* qk_scale,
+                                   long long lds, const void* vt8, const void* v_scale, void* const* out_peers, long long ldo,
+                                   int Lq, int Lk, int heads, float scale, int world, int rank, int Lp, int flags, void* ws,
+                                   long long ws_bytes, void* stream_) {
+  using namespace yb;
+  if (!out_peers || world < 2 || world > 8 || rank < 0 || rank >= world || Lp <= 0) return YB_ERR_ARG;
+  if (Lq != world * Lp || Lk > Lq) return YB_ERR_ARG;
+  Att8Peers sp = {};
+  for (int i = 0; i < world; ++i) {
+    if (!out_peers[i]) return YB_ERR_ARG;
+    if (reinterpret_cast<uintptr_t>(out_peers[i]) & 0xF) return YB_ERR_ALIGNMENT;
+    sp.out[i] = static_cast<__nv_bfloat16*>(out_peers[i]);
+  }
+  sp.world = world;
+  sp.rank = rank;
+  sp.Lp = Lp;
+  return launch_attention_fp8(q8, ldq, k8, ldk, qk_scale, lds, vt8, v_scale, out_peers[rank], ldo, Lq, Lk, heads, scale, flags,
+                              ws, ws_bytes, &sp, stream_);
 }

@@ -3,6 +3,7 @@
 // and the small fp32 linears the reference keeps in fp32 (time MLP, head).
 #include "yb_host.h"
 #include "yb_ptx.cuh"
+#include "../../include/yume_b200_fp8_sp.h"
 
 namespace yb {
 
@@ -385,7 +386,9 @@ struct PeerPtrs {
 struct PeerPtrsF {
   float* p[8];
 };
-template <int NCH>
+// LOCAL (yb_sp_pack_qkv, the NCCL transport): the same rows stored into this rank's own send buffer [P(owner), Lp, 3 Wh] =
+// peers.p[0], the chunk of owner p at block p, instead of into block `rank` of owner p's receive buffer
+template <int NCH, bool LOCAL>
 __global__ void __launch_bounds__(256)
 sp_scatter_qkv_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const float* __restrict__ wq,
                       const float* __restrict__ wk, const float2* __restrict__ rope, int rope_len, int L, int D,
@@ -447,7 +450,10 @@ sp_scatter_qkv_kernel(const __nv_bfloat16* __restrict__ qkv, long long ld, const
         o = make_uint4(ov[0], ov[1], ov[2], ov[3]);
       }
       const int peer = col / Wh;
-      *reinterpret_cast<uint4*>(peers.p[peer] + dst_row + part * Wh + (col - peer * Wh)) = o;
+      if (LOCAL)
+        *reinterpret_cast<uint4*>(peers.p[0] + (static_cast<long long>(peer) * Lp + row) * W3 + part * Wh + (col - peer * Wh)) = o;
+      else
+        *reinterpret_cast<uint4*>(peers.p[peer] + dst_row + part * Wh + (col - peer * Wh)) = o;
     }
   }
 }
@@ -868,7 +874,7 @@ extern "C" int yb_sp_scatter_qkv(const void* qkv, long long ld, const void* wq, 
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
 #define YB_SC(NCH)                                                                                                   \
   if (C == (NCH) * 256) {                                                                                            \
-    sp_scatter_qkv_kernel<NCH><<<(L + 7) / 8, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(qkv), ld,                \
+    sp_scatter_qkv_kernel<NCH, false><<<(L + 7) / 8, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(qkv), ld,                \
                                                           static_cast<const float*>(wq), static_cast<const float*>(wk), \
                                                           static_cast<const float2*>(rope), rope_len, L, D, eps, pp,   \
                                                           rank, Lp, Wh);                                              \
@@ -879,5 +885,30 @@ extern "C" int yb_sp_scatter_qkv(const void* qkv, long long ld, const void* wq, 
   YB_SC(4)
   YB_SC(1)
 #undef YB_SC
+  return YB_ERR_SHAPE;
+}
+
+extern "C" int yb_sp_pack_qkv(const void* qkv, long long ld, const void* wq, const void* wk, const void* rope, int rope_len,
+                              int L, int C, int D, float eps, void* send, int world, int Lp, void* stream_) {
+  if (!qkv || !wq || !wk || !send || L <= 0 || world < 2 || world > 8 || Lp < L) return YB_ERR_ARG;
+  if (C % (world * D) != 0 || (ld % 8)) return YB_ERR_SHAPE;
+  if (reinterpret_cast<uintptr_t>(send) & 0xF) return YB_ERR_ALIGNMENT;
+  PeerPtrs dst = {};
+  dst.p[0] = static_cast<__nv_bfloat16*>(send);
+  const int Wh = C / world;
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+#define YB_PK(NCH)                                                                                                   \
+  if (C == (NCH) * 256) {                                                                                            \
+    sp_scatter_qkv_kernel<NCH, true><<<(L + 7) / 8, 256, 0, s>>>(static_cast<const __nv_bfloat16*>(qkv), ld,           \
+                                                                static_cast<const float*>(wq), static_cast<const float*>(wk), \
+                                                                static_cast<const float2*>(rope), rope_len, L, D, eps, dst, \
+                                                                0, Lp, Wh);                                                 \
+    return check_launch("sp_pack_qkv");                                                                              \
+  }
+  YB_PK(12)
+  YB_PK(20)
+  YB_PK(4)
+  YB_PK(1)
+#undef YB_PK
   return YB_ERR_SHAPE;
 }

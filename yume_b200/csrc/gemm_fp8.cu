@@ -19,6 +19,7 @@
 #include "yb_host.h"
 #include "../../include/yume_b200_fp8.h"
 #include "../../include/yume_b200_fp8_vae.h"
+#include "../../include/yume_b200_fp8_sp.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -471,6 +472,32 @@ quant_rows_fp8_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, uint8_
   }
 }
 
+// quant_rows_fp8_kernel over a K-split source (yb_quant_rows_fp8_split): group g of row m lies in chunk (g * 128) / split, at
+// column (g * 128) % split of that chunk's row m; the arithmetic per group is quant_rows_fp8_kernel's
+__global__ void __launch_bounds__(256)
+quant_rows_fp8_split_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, int split, long long split_stride,
+                            uint8_t* __restrict__ out, long long ldo, float* __restrict__ out_scale, long long lds, int M,
+                            int groups) {
+  const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (row >= M) return;
+  const __nv_bfloat16* xr = x + static_cast<long long>(row) * ldx + lane * 4;
+  uint8_t* orow = out + static_cast<long long>(row) * ldo + lane * 4;
+  const int per_chunk = split >> 7;
+  for (int g = 0; g < groups; ++g) {
+    const int chunk = g / per_chunk;
+    const uint2 raw = __ldg(reinterpret_cast<const uint2*>(xr + chunk * split_stride + (g - chunk * per_chunk) * 128));
+    const float2 a = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.x));
+    const float2 b = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&raw.y));
+    const float4 y = make_float4(a.x, a.y, b.x, b.y);
+    const float amax = f8_warp_max(amax4(y.x, y.y, y.z, y.w));
+    float inv, scale;
+    group_scale(amax, inv, scale);
+    store_e4m3x4(orow + g * 128, y, inv);
+    if (lane == 0) out_scale[static_cast<long long>(g) * lds + row] = scale;
+  }
+}
+
 // 4-D e4m3 tensor map over a dense channels-last volume [T, H, W, C] (C bytes per voxel), box {128 channels, bw, bh, bt}, 128-byte
 // swizzle, out-of-bounds voxels read as zeros
 static int make_tmap_e4m3_4d(CUtensorMap* tm, const void* base, uint64_t T, uint64_t H, uint64_t W, uint64_t C, uint32_t bt,
@@ -649,4 +676,18 @@ extern "C" int yb_quant_rows_fp8(const void* x, long long ldx, void* out, long l
   quant_rows_fp8_kernel<<<(M + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const __nv_bfloat16*>(x), ldx, static_cast<uint8_t*>(out), ldo, static_cast<float*>(out_scale), lds, M, K / 128);
   return check_launch("quant_rows_fp8");
+}
+
+extern "C" int yb_quant_rows_fp8_split(const void* x, long long ldx, int split, long long split_stride, void* out, long long ldo,
+                                       void* out_scale, long long lds, int M, int K, void* stream_) {
+  using namespace yb;
+  if (!x || !out || !out_scale || M <= 0 || K <= 0 || split <= 0 || lds < M) return YB_ERR_ARG;
+  if (K % 128 != 0 || split % 128 != 0 || K % split != 0) return YB_ERR_SHAPE;
+  if ((ldx % 8) || (split_stride % 8) || (ldo % 16) || (lds % 4) || (reinterpret_cast<uintptr_t>(x) & 0xF) ||
+      (reinterpret_cast<uintptr_t>(out) & 0xF) || (reinterpret_cast<uintptr_t>(out_scale) & 0x3))
+    return YB_ERR_ALIGNMENT;
+  quant_rows_fp8_split_kernel<<<(M + 7) / 8, 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const __nv_bfloat16*>(x), ldx, split, split_stride, static_cast<uint8_t*>(out), ldo,
+      static_cast<float*>(out_scale), lds, M, K / 128);
+  return check_launch("quant_rows_fp8_split");
 }

@@ -141,9 +141,11 @@ inline int check_launch(const char* what) {
 }
 
 // attention.cu: merge the KV-segment partials (O in true units [tail * ns, 256, 128], then (row max log2, row sum)
-// [tail * ns, 256, 2]) of the `tail` units after the first `full_units` and store bf16 rows of out (see yb_attention_plan)
+// [tail * ns, 256, 2]) of the `tail` units after the first `full_units` and store bf16 rows of out (see yb_attention_plan).
+// world > 1: row g goes to row rank * Lp + g % Lp of out_peers[g / Lp] instead, as yb_attention_sp stores it.
 int attention_combine_launch(void* out, long long ldo, int Lq, int nq, int full_units, int ns, int tail, float* ws_o,
-                             float* ws_ml, cudaStream_t stream);
+                             float* ws_ml, cudaStream_t stream, void* const* out_peers = nullptr, int world = 1, int rank = 0,
+                             int Lp = 0);
 
 constexpr int kMaxDevices = 64;
 inline int current_device() {

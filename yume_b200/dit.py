@@ -266,13 +266,20 @@ class WanDiT:
         QKV GEMM itself (yb_gemm_sp_qkv: peer stores under the main loop, normalisation finished on the receiver);
         "nccl" = NCCL all_to_all_single; "auto" = p2p when symmetric memory is available. For the NCCL path builds the peer-major fused q|k|v weight:
         rows ordered [peer p][q, k, v][heads p*H/P .. (p+1)*H/P) so that the QKV GEMM's `n_split` epilogue emits
-        exactly the chunks the all-to-all sends."""
+        exactly the chunks the all-to-all sends.
+        precision "fp8" / "fp8_attn" run "p2p", "nccl" and "auto" (DESIGN.md §6): the q|k|v GEMM writes the standard [Lp, 3C]
+        rows and one norm + RoPE pass scatters them (p2p) or packs them into the NCCL send buffer, so no peer-major weight is built;
+        "p2p_gemm" is the bf16 GEMM with the exchange in its epilogue and has no e4m3 form."""
         if transport not in ("auto", "p2p", "p2p_gemm", "nccl"):
             raise YumeB200Error("transport must be auto, p2p, p2p_gemm or nccl")
-        if self._fp8:
-            raise YumeB200Error("sequence parallelism runs the bf16 block GEMMs only: build the engine with precision='bf16'")
-        self.sp_transport, self._sp_p2p = transport, None
         import torch.distributed as dist
+        if self._fp8:
+            if transport == "p2p_gemm":
+                raise YumeB200Error(f"transport 'p2p_gemm' fuses the exchange into the bf16 q|k|v GEMM, which has no e4m3 form: "
+                                    f"use 'p2p', 'nccl' or 'auto' with precision={self.precision!r}")
+            if group is None and not (dist.is_available() and dist.is_initialized()):
+                raise YumeB200Error("sequence parallelism needs an initialised torch.distributed process group")
+        self.sp_transport, self._sp_p2p = transport, None
         P = dist.get_world_size(group)
         if self.heads % P:
             raise YumeB200Error(f"{self.heads} heads do not divide over {P} ranks")
@@ -283,9 +290,10 @@ class WanDiT:
             self._build_nccl_weights()
 
     def _build_nccl_weights(self) -> None:
-        """Peer-major copies of the fused q|k|v weights: only the NCCL transport reads them (+6.3 GB at 14B), so they are
-        built when that transport is chosen — up front, or when symmetric memory turns out to be unavailable."""
-        if "w_qkv_sp" in self.blocks[0]:
+        """Peer-major copies of the fused q|k|v weights: only the bf16 NCCL transport reads them (+6.3 GB at 14B), so they are
+        built when that transport is chosen — up front, or when symmetric memory turns out to be unavailable. The fp8 engine
+        packs the send buffer from the standard q|k|v rows instead (yb_sp_pack_qkv) and never builds them."""
+        if self._fp8 or "w_qkv_sp" in self.blocks[0]:
             return
         idx = sp_qkv_row_order(self.dim, self.heads, self.sp_world).to(self.device)
         for b in self.blocks:
@@ -510,21 +518,38 @@ class WanDiT:
         else:
             qkv = self._buf("qkv", (Lp, 3 * C), _BF16)
             T.begin("gemm_qkv")
-            ops.gemm(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
+            self._linear(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
             T.end("gemm_qkv")
             T.begin("sp_scatter_qkv")
             ops.sp_scatter_qkv(qkv, b["nq"], b["nk"], rope, rope_len, D, self.eps, st["qkv_ptrs"][par], self.sp_rank, Lp)
             st["hdl"].barrier(channel=0)
             T.end("sp_scatter_qkv")
         T.begin("self_attention")
-        ops.attention_sp(full[:, :Wh], full[:L_true, Wh:2 * Wh], full[:L_true, 2 * Wh:], st["att_ptrs"][par], Wh, Hp,
-                         self.sp_rank, Lp)
+        if self.precision == "fp8_attn":
+            qk8, qk_s, vt8, v_s = self._quant_qkv8(full, L_true, Hp)
+            ops.attention_fp8_sp(qk8[:, :Wh], qk8[:L_true, Wh:], qk_s, vt8, v_s, st["att_ptrs"][par], Wh, Hp, self.sp_rank, Lp)
+        else:
+            ops.attention_sp(full[:, :Wh], full[:L_true, Wh:2 * Wh], full[:L_true, 2 * Wh:], st["att_ptrs"][par], Wh, Hp,
+                             self.sp_rank, Lp)
         st["hdl"].barrier(channel=0)
         T.end("self_attention")
         T.begin("gemm_o")
-        ops.gemm(st["att"][par], b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx,
-                 a_split=Wh, a_split_stride=Lp * Wh, shape=(Lp, C))
+        self._o_proj_sp(st["att"][par], b, xs, m, tok_idx)
         T.end("gemm_o")
+
+    def _o_proj_sp(self, att: Tensor, b: dict, xs: Tensor, m: Tensor, tok_idx: Optional[Tensor]) -> None:
+        """The o projection (GATE_RES into this rank's xs) of the exchanged attention output att [P, Lp, heads/P*128], whose
+        K-split layout holds row t of the [Lp, C] input as P chunks Lp*Wh apart: the bf16 GEMM reads it through a 3-D map (a_split);
+        under fp8 one split quantiser gathers it into the e4m3 pair the fp8 GEMM reads (the one-GPU path's quantiser launch)."""
+        P, Lp, Wh = att.shape
+        C = self.dim
+        if self._fp8:
+            a8 = self._act8("att8", Lp, C)
+            ops.quant_rows_fp8_split(att, *a8, Wh, Lp * Wh, (Lp, C))
+            ops.gemm_fp8(*a8, *b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx)
+            return
+        ops.gemm(att, b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx,
+                 a_split=Wh, a_split_stride=Lp * Wh, shape=(Lp, C))
 
     def _self_attention_sp(self, i: int, b: dict, h: Tensor, xs: Tensor, m: Tensor, tok_idx: Optional[Tensor], rope: Tensor,
                            rope_len: int, L_true: int) -> None:
@@ -546,13 +571,23 @@ class WanDiT:
         T = self.timer
         send = self._buf("sp_qkv_send", (P, Lp, W3), _BF16)
         recv = self._buf("sp_qkv_recv", (P, Lp, W3), _BF16)
-        T.begin("gemm_qkv")
-        ops.gemm(h, b["w_qkv_sp"], b["b_qkv_sp"], send, ops.YB_EPI_BF16, n_split=W3, split_stride=Lp * W3, shape=(Lp, C))
-        T.end("gemm_qkv")
-        T.begin("qk_norm_rope")
-        ops.qk_norm_rope(send[0], send[0][:, Wh:], b["nq"], b["nk"], rope, D, self.eps, rope_len,
-                         pieces=(Lp, C, Wh, Lp * W3))
-        T.end("qk_norm_rope")
+        if self._fp8:
+            # standard [Lp, 3C] rows from the e4m3 GEMM, then yb_sp_scatter_qkv's norm + RoPE with the send buffer as destination
+            qkv = self._buf("qkv", (Lp, 3 * C), _BF16)
+            T.begin("gemm_qkv")
+            self._linear(h, b["w_qkv"], b["b_qkv"], qkv, ops.YB_EPI_BF16)
+            T.end("gemm_qkv")
+            T.begin("qk_norm_rope")
+            ops.sp_pack_qkv(qkv, b["nq"], b["nk"], rope, rope_len, D, self.eps, send)
+            T.end("qk_norm_rope")
+        else:
+            T.begin("gemm_qkv")
+            ops.gemm(h, b["w_qkv_sp"], b["b_qkv_sp"], send, ops.YB_EPI_BF16, n_split=W3, split_stride=Lp * W3, shape=(Lp, C))
+            T.end("gemm_qkv")
+            T.begin("qk_norm_rope")
+            ops.qk_norm_rope(send[0], send[0][:, Wh:], b["nq"], b["nk"], rope, D, self.eps, rope_len,
+                             pieces=(Lp, C, Wh, Lp * W3))
+            T.end("qk_norm_rope")
         T.begin("sp_all_to_all_qkv")
         dist.all_to_all_single(recv, send, group=self.sp_group)
         T.end("sp_all_to_all_qkv")
@@ -560,14 +595,13 @@ class WanDiT:
         att_send = self._buf("sp_att_send", (P, Lp, Wh), _BF16)
         att_recv = self._buf("sp_att_recv", (P, Lp, Wh), _BF16)
         T.begin("self_attention")
-        ops.attention(full[:, :Wh], full[:L_true, Wh:2 * Wh], full[:L_true, 2 * Wh:], att_send.view(P * Lp, Wh), Hp)
+        self._attention(full, att_send.view(P * Lp, Wh), L_true, Hp)
         T.end("self_attention")
         T.begin("sp_all_to_all_out")
         dist.all_to_all_single(att_recv, att_send, group=self.sp_group)
         T.end("sp_all_to_all_out")
         T.begin("gemm_o")
-        ops.gemm(att_recv, b["w_o"], b["b_o"], xs, ops.YB_EPI_GATE_RES, gate=m[:, 2], tok_idx=tok_idx,
-                 a_split=Wh, a_split_stride=Lp * Wh, shape=(Lp, C))
+        self._o_proj_sp(att_recv, b, xs, m, tok_idx)
         T.end("gemm_o")
 
     def _cross_kv(self, ctx: Tensor, own_storage: bool = False, block: Optional[int] = None):
@@ -736,23 +770,30 @@ class WanDiT:
         ops.gemm(h, b["w1"], b["b1"], hid, ops.YB_EPI_GELU_BF16)
         return hid
 
-    def _attention(self, qkv: Tensor, att: Tensor, k_len: int) -> None:
+    def _attention(self, qkv: Tensor, att: Tensor, k_len: int, heads: Optional[int] = None) -> None:
         """Self-attention of the normed, roped q|k|v rows over the first k_len rows as keys, into bf16 `att`. "fp8_attn" runs
         it on e4m3 operands (include/yume_b200_fp8_attn.h): q and k are quantised by one launch over the [L, 2C] view (a 1x128
         group is one head of one token: q scales of head h at scale row h, k scales at heads + h), v transposed per (head,
-        128-key tile)."""
-        C, H = self.dim, self.heads
+        128-key tile). heads: the heads the rows hold (default all; heads/P on a Ulysses rank's exchanged rows)."""
+        H = self.heads if heads is None else heads
+        C = H * self.head_dim
         if self.precision != "fp8_attn":
             ops.attention(qkv[:, :C], qkv[:k_len, C:2 * C], qkv[:k_len, 2 * C:], att, H)
             return
-        L = qkv.shape[0]
+        qk8, qk_s, vt8, v_s = self._quant_qkv8(qkv, k_len, H)
+        ops.attention_fp8(qk8[:, :C], qk8[:k_len, C:], qk_s, vt8, v_s, att, H)
+
+    def _quant_qkv8(self, qkv: Tensor, k_len: int, H: int):
+        """The e4m3 operands of the fp8 attention from bf16 q|k|v rows [L, 3 H 128]: (qk8, qk_s) of the [L, 2 H 128] q|k view, and
+        v's first k_len rows transposed (vt8, v_s)."""
+        L, C = qkv.shape[0], H * self.head_dim
         Lkp = ops.vt8_keys(k_len)
         qk8, qk_s = self._act8("qk8", L, 2 * C)
         vt8 = self._buf("vt8", (H, 128, Lkp), torch.float8_e4m3fn)
         v_s = self._buf("vt8_s", (H, Lkp // 128), _F32)
         ops.quant_rows_fp8(qkv[:, :2 * C], qk8, qk_s)
         ops.quant_vt_fp8(qkv[:k_len, 2 * C:], vt8, v_s, H)
-        ops.attention_fp8(qk8[:, :C], qk8[:k_len, C:], qk_s, vt8, v_s, att, H)
+        return qk8, qk_s, vt8, v_s
 
     def weight_bytes(self) -> int:
         """Bytes of every weight tensor the engine holds on its device (bench and tests compare the two precisions)."""

@@ -973,6 +973,76 @@ def attention_fp8(q8: torch.Tensor, k8: torch.Tensor, qk_scale: torch.Tensor, vt
 
 
 # ------------------------------------------------------------------------------------------------------------
+# FP8 under Ulysses sequence parallelism (include/yume_b200_fp8_sp.h): the fp8 quantiser and attention with the exchange's
+# layouts, and the NCCL send-buffer pack of the q|k|v rows
+# ------------------------------------------------------------------------------------------------------------
+def quant_rows_fp8_split(x: torch.Tensor, out: torch.Tensor, out_scale: torch.Tensor, split: int, split_stride: int,
+                         shape: tuple) -> torch.Tensor:
+    """quant_rows_fp8 of the [M, K] matrix (shape) that x holds as K / split chunks `split_stride` elements apart (x is the
+    first chunk's [M, split] rows, e.g. the [P, Lp, Wh] exchange buffer) -> out e4m3 [M, K] + out_scale f32 [K/128, >= M]."""
+    global _launches
+    _need(x, torch.bfloat16, "x")
+    _need(out, _E4M3, "out")
+    _need(out_scale, torch.float32, "out_scale")
+    M, K = shape
+    if tuple(out.shape) != (M, K) or out_scale.shape[0] != K // 128:
+        raise YumeB200Error(f"quant_rows_fp8_split: out must be [{M}, {K}] and out_scale [{K // 128}, >= {M}]")
+    check(_lib.load().yb_quant_rows_fp8_split(x.data_ptr(), x.stride(-2), split, split_stride, out.data_ptr(), out.stride(0),
+                                              out_scale.data_ptr(), out_scale.stride(0), M, K, _stream()),
+          "yb_quant_rows_fp8_split")
+    _launches += 1
+    return out
+
+
+def attention_fp8_sp(q8: torch.Tensor, k8: torch.Tensor, qk_scale: torch.Tensor, vt8: torch.Tensor, v_scale: torch.Tensor,
+                     out_peer_ptrs, ldo: int, heads: int, rank: int, Lp: int, scale: Optional[float] = None,
+                     split: int = 0) -> None:
+    """attention_fp8 over the P*Lp gathered query rows whose output row g is stored into row rank*Lp + g % Lp of peer g // Lp's
+    [P, Lp, heads*128] receive buffer (out_peer_ptrs: one device address per rank, row stride ldo)."""
+    global _launches, _flops
+    for n, t in (("q8", q8), ("k8", k8), ("vt8", vt8)):
+        _need(t, _E4M3, n)
+    _need(qk_scale, torch.float32, "qk_scale")
+    _need(v_scale, torch.float32, "v_scale")
+    Lq, Lk = q8.shape[0], k8.shape[0]
+    Lkp = vt8_keys(Lk)
+    if q8.shape[1] != heads * 128 or k8.shape[1] != heads * 128 or qk_scale.shape[0] != 2 * heads:
+        raise YumeB200Error("attention_fp8_sp supports head_dim 128 only, with qk_scale [2*heads, >= Lq]")
+    if tuple(vt8.shape) != (heads, 128, Lkp) or tuple(v_scale.shape) != (heads, Lkp // 128):
+        raise YumeB200Error("attention_fp8_sp: vt8 / v_scale do not match Lk and heads")
+    if scale is None:
+        scale = 1.0 / math.sqrt(128.0)
+    flags = (split & 7) << 4
+    ws, ws_bytes = _attention_ws(Lq, Lk, heads, flags, q8.device)
+    check(_lib.load().yb_attention_fp8_sp(q8.data_ptr(), q8.stride(0), k8.data_ptr(), k8.stride(0), qk_scale.data_ptr(),
+                                          qk_scale.stride(0), vt8.data_ptr(), v_scale.data_ptr(), _ptr_array(out_peer_ptrs), ldo,
+                                          Lq, Lk, heads, scale, len(out_peer_ptrs), rank, Lp, flags, _ptr(ws), ws_bytes,
+                                          _stream()), "yb_attention_fp8_sp")
+    _launches += 1
+    _flops += 4.0 * Lq * Lk * heads * 128
+
+
+def sp_pack_qkv(qkv: torch.Tensor, wq: torch.Tensor, wk: torch.Tensor, rope: Optional[torch.Tensor], rope_len: int,
+                head_dim: int, eps: float, send: torch.Tensor) -> None:
+    """qkv bf16 [L_local, 3C] -> RMSNorm/RoPE on q, k and the q|k|v chunks of every owner rank's heads packed into this rank's
+    send buffer bf16 [P, Lp, 3C/P] (the operand of the NCCL all-to-all)."""
+    global _launches
+    _need(qkv, torch.bfloat16, "qkv")
+    _need(send, torch.bfloat16, "send")
+    _need(wq, torch.float32, "wq")
+    _need(wk, torch.float32, "wk")
+    L, C3 = qkv.shape
+    P, Lp, W3 = send.shape
+    if not send.is_contiguous() or P * W3 != C3:
+        raise YumeB200Error(f"sp_pack_qkv: send must be a contiguous [P, Lp, {C3} / P]")
+    if rope is not None:
+        _need(rope, torch.float32, "rope")
+    check(_lib.load().yb_sp_pack_qkv(qkv.data_ptr(), qkv.stride(0), wq.data_ptr(), wk.data_ptr(), _ptr(rope), rope_len, L,
+                                     C3 // 3, head_dim, eps, send.data_ptr(), P, Lp, _stream()), "yb_sp_pack_qkv")
+    _launches += 1
+
+
+# ------------------------------------------------------------------------------------------------------------
 # FP8 Wan2.2 VAE decode convs (include/yume_b200_fp8_vae.h). An fp8 activation stream is a pair: e4m3 values [T, H, W, Cp] and
 # f32 scales [T, Cp / 128, H, W], one per voxel and 128-channel group (frame-major: a frame of both is one contiguous block).
 # ------------------------------------------------------------------------------------------------------------
