@@ -181,6 +181,16 @@ RESUME_SIGNATURES = {
     "yb_vae_frame_match": (_i, [_vp, _i, _vp, _i, _i, _ll, _i, _vp, _vp]),
 }
 
+# every symbol include/yume_b200_vae_rows.h declares (the row-band forms of a row-parallel Wan VAE decode)
+ROWS_SIGNATURES = {
+    "yb_conv3d_rows": (_i, [C.POINTER(Conv3dArgs), _i, _vp]),
+    "yb_vae_rms_act_rows": (_i, [_vp, _ll, _vp, _vp, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+    "yb_vae_rows_pack": (_i, [_vp, _vp, _i, _i, _ll, _vp]),
+    "yb_vae_rows_unpack": (_i, [_vp, _vp, _vp, _i, _i, _ll, _vp]),
+    "yb_vae_unpatchify2_clamp_rows": (_i, [_vp, _ll, _vp, _ll, _ll, _i, _i, _i, _vp]),
+    "yb_nhwc_to_nchw_f32_clamp_rows": (_i, [_vp, _ll, _vp, _ll, _ll, _i, _i, _i, _i, _f, _f, _vp]),
+}
+
 _lib = None
 
 
@@ -203,7 +213,7 @@ def load():
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
                               **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES, **RESUME_SIGNATURES,
-                              **FP8_SP_SIGNATURES}.items():
+                              **FP8_SP_SIGNATURES, **ROWS_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

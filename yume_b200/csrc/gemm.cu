@@ -28,6 +28,7 @@
 // and HALF of the B tile, and multicasts that half into both CTAs, so the B operand crosses L2 once per pair of SMs.
 #include "yb_host.h"
 #include "../../include/yume_b200_stream.h"
+#include "../../include/yume_b200_vae_rows.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -1008,7 +1009,9 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
 // Causal 3x3x3 conv (replicate padding) as an implicit GEMM on the same kernel. See include/yume_b200.h.
 // t_hist > 0 is the history form (include/yume_b200_stream.h): the input holds t_hist carried frames in front of the T new ones,
 // and those frames take the place of the causal zero padding in time (the tensor map spans all t_hist + T frames).
-static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
+// rows is the row-halo form (include/yume_b200_vae_rows.h): the input has H + 2 rows, the two outer ones the neighbours' halo
+// rows, and output row h reads input rows h .. h + 2 (no zero fill in H; the tile plan is the one of the H output rows).
+static int conv3d_launch(const yb_conv3d_args* a, int t_hist, bool rows, void* stream_) {
   using namespace yb;
   if (!a || !a->xpad || !a->w || !a->out) return YB_ERR_ARG;
   if (a->struct_bytes != sizeof(yb_conv3d_args)) return YB_ERR_ARG;
@@ -1033,6 +1036,7 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
   if (strided && !a->oob_zero_pad) return YB_ERR_ARG;
   // history: exactly the kt-1 frames of the causal pad (unit stride), or the one frame the stride-2 time_conv carries
   if (t_hist > 0 && (!a->oob_zero_pad || t_hist != (st_t > 1 ? 1 : kt - 1))) return YB_ERR_ARG;
+  if (rows && (!a->oob_zero_pad || strided || kh != 3)) return YB_ERR_ARG;
   const int inT = a->T + t_hist;   // frames the tensor map spans
   int oT = a->T, oH = a->H, oW = a->W;
   if (st_t > 1) oT = (inT - kt) / st_t + 1;
@@ -1051,7 +1055,7 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
   p.kh = kh; p.kw = kw;
   p.st_t = st_t; p.st_h = st_hw; p.st_w = st_hw;
   p.off_t = (a->oob_zero_pad && st_t == 1) ? kt - 1 - t_hist : 0;
-  p.off_h = (a->oob_zero_pad && st_hw == 1) ? kh / 2 : 0;
+  p.off_h = (a->oob_zero_pad && st_hw == 1 && !rows) ? kh / 2 : 0;
   p.off_w = (a->oob_zero_pad && st_hw == 1) ? kw / 2 : 0;
   p.out_t_mul = a->out_t_mul > 0 ? a->out_t_mul : 1;
   p.out_t_add = a->out_t_add;
@@ -1068,7 +1072,7 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
   p.res_ld = a->res_ld;
   CUtensorMap tmA, tmB;
   const int padT = a->oob_zero_pad ? 0 : kt - 1, padH = a->oob_zero_pad ? 0 : kh - 1, padW = a->oob_zero_pad ? 0 : kw - 1;
-  int rc = make_tmap_bf16_4d(&tmA, a->xpad, inT + padT, a->H + padH, a->W + padW, a->Cp, p.TT, p.TH,
+  int rc = make_tmap_bf16_4d(&tmA, a->xpad, inT + padT, a->H + (rows ? 2 : padH), a->W + padW, a->Cp, p.TT, p.TH,
                              fuse_w ? CONVW_ROWS : p.TW, 64, st_t, st_hw, st_hw);
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmB, a->w, a->Cout, static_cast<uint64_t>(taps) * a->Cp, static_cast<uint64_t>(taps) * a->Cp,
@@ -1103,9 +1107,13 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, void* stream_) {
 #undef YB_CONV_DISPATCH
 }
 
-extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream) { return conv3d_launch(a, 0, stream); }
+extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream) { return conv3d_launch(a, 0, false, stream); }
 
 extern "C" int yb_conv3d_causal_hist(const yb_conv3d_args* a, int t_hist, void* stream) {
   if (t_hist <= 0) return YB_ERR_ARG;
-  return conv3d_launch(a, t_hist, stream);
+  return conv3d_launch(a, t_hist, false, stream);
+}
+
+extern "C" int yb_conv3d_rows(const yb_conv3d_args* a, int t_hist, void* stream) {
+  return conv3d_launch(a, t_hist, true, stream);
 }

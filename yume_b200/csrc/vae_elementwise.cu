@@ -10,6 +10,7 @@
 #include "../../include/yume_b200_stream.h"
 #include "../../include/yume_b200_fp8_vae.h"
 #include "../../include/yume_b200_vae_resume.h"
+#include "../../include/yume_b200_vae_rows.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -314,10 +315,12 @@ __global__ void __launch_bounds__(256) vae_assemble_tiles_kernel(const TileAsm a
 // ---------------------------------------------------------------------------------------------------------
 // NCH = 16-byte chunks per lane per voxel, G = lanes per voxel (G < 32 only with NCH == 1: narrow rows share a warp).
 // A warp keeps U * (32 / G) voxels in flight, U = 4 / NCH. All index math is 32-bit and the f == 1 path has none.
-template <int NCH, int G>
+// BAND (yb_vae_rms_act_rows): out is a band buffer [T, H + 2, W, Cp] written at rows 1 .. H, and the first and last written row of
+// every frame also go to send [2, T, W, Cp] when it is not NULL; the values are those of the dense form.
+template <int NCH, int G, bool BAND = false>
 __global__ void __launch_bounds__(256)
 rms_act_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16* __restrict__ out, const float* __restrict__ gamma,
-               int T, int Hs, int Ws, int C, int Cp, int f, int silu) {
+               int T, int Hs, int Ws, int C, int Cp, int f, int silu, __nv_bfloat16* __restrict__ send = nullptr) {
   constexpr int U = 4 / NCH;
   constexpr int SUB = 32 / G;                     // voxels side by side in one warp
   constexpr int VPI = U * SUB;                    // voxels per warp iteration
@@ -400,7 +403,17 @@ rms_act_kernel(const __nv_bfloat16* __restrict__ x, long long ldx, __nv_bfloat16
           }
           o = make_uint4(pack_bf16x2(y[0], y[1]), pack_bf16x2(y[2], y[3]), pack_bf16x2(y[4], y[5]), pack_bf16x2(y[6], y[7]));
         }
-        *reinterpret_cast<uint4*>(out + static_cast<long long>(v) * Cp + c * 8) = o;
+        if constexpr (BAND) {
+          const int w = v % W, r = v / W;
+          const int h = r % H, t = r / H;
+          *reinterpret_cast<uint4*>(out + (static_cast<long long>(t * (H + 2) + h + 1) * W + w) * Cp + c * 8) = o;
+          if (send) {
+            if (h == 0) *reinterpret_cast<uint4*>(send + (static_cast<long long>(t) * W + w) * Cp + c * 8) = o;
+            if (h == H - 1) *reinterpret_cast<uint4*>(send + (static_cast<long long>(T + t) * W + w) * Cp + c * 8) = o;
+          }
+        } else {
+          *reinterpret_cast<uint4*>(out + static_cast<long long>(v) * Cp + c * 8) = o;
+        }
       }
     }
   }
@@ -644,6 +657,64 @@ __global__ void unpatchify2_clamp_kernel(const float* __restrict__ y, long long 
     const int q = ho & 1, r = wo & 1;
     const float val = y[((static_cast<long long>(f) * H + (ho >> 1)) * W + (wo >> 1)) * ldy + (c * 2 + r) * 2 + q];
     out[c * plane + (i - static_cast<long long>(c) * T * (2 * H) * (2 * W))] = fminf(fmaxf(val, -1.f), 1.f);
+  }
+}
+
+// Row-band form of unpatchify2_clamp_kernel (include/yume_b200_vae_rows.h): the band's 2Hs rows of T frames, frames `frame`
+// elements apart, rows 2W apart
+__global__ void unpatchify2_clamp_rows_kernel(const float* __restrict__ y, long long ldy, float* __restrict__ out, int T, int Hs,
+                                              int W, long long plane, long long frame) {
+  const long long total = 3LL * T * (2 * Hs) * (2 * W);
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int wo = static_cast<int>(i % (2 * W));
+    long long v = i / (2 * W);
+    const int ho = static_cast<int>(v % (2 * Hs));
+    v /= (2 * Hs);
+    const int f = static_cast<int>(v % T);
+    const int c = static_cast<int>(v / T);
+    const int q = ho & 1, r = wo & 1;
+    const float val = y[((static_cast<long long>(f) * Hs + (ho >> 1)) * W + (wo >> 1)) * ldy + (c * 2 + r) * 2 + q];
+    out[c * plane + f * frame + static_cast<long long>(ho) * (2 * W) + wo] = fminf(fmaxf(val, -1.f), 1.f);
+  }
+}
+
+// Row-band form of nhwc_to_nchw_kernel: x f32 [T*Hs*W, ldx] -> Cn channels x T frames (`frame` apart) x Hs rows x W columns
+__global__ void nhwc_to_nchw_rows_kernel(const float* __restrict__ x, long long ldx, float* __restrict__ out, int T, int Hs, int W,
+                                         int Cn, float lo, float hi, long long plane, long long frame) {
+  const long long N = static_cast<long long>(T) * Hs * W;
+  const long long total = N * Cn;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long v = i % N;
+    const int c = static_cast<int>(i / N);
+    const long long f = v / (static_cast<long long>(Hs) * W), hw = v % (static_cast<long long>(Hs) * W);
+    out[c * plane + f * frame + hw] = fminf(fmaxf(x[v * ldx + c], lo), hi);
+  }
+}
+
+// Halo glue of a band buffer [T, Hs + 2, nvec] (16-byte words): pack copies rows 1 and Hs into send [2, T, nvec]; unpack copies
+// recv_top / recv_bot [T, nvec] into rows 0 and Hs + 1, zeros for a NULL source
+__global__ void rows_pack_kernel(const uint4* __restrict__ buf, uint4* __restrict__ send, int T, int Hs, long long nvec) {
+  const long long total = 2LL * T * nvec;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long e = i % nvec, r = i / nvec;
+    const int t = static_cast<int>(r % T), side = static_cast<int>(r / T);
+    send[i] = buf[(static_cast<long long>(t) * (Hs + 2) + (side ? Hs : 1)) * nvec + e];
+  }
+}
+
+__global__ void rows_unpack_kernel(const uint4* __restrict__ top, const uint4* __restrict__ bot, uint4* __restrict__ buf, int T,
+                                   int Hs, long long nvec) {
+  const long long total = 2LL * T * nvec;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const long long e = i % nvec, r = i / nvec;
+    const int t = static_cast<int>(r % T), side = static_cast<int>(r / T);
+    const uint4* src = side ? bot : top;
+    buf[(static_cast<long long>(t) * (Hs + 2) + (side ? Hs + 1 : 0)) * nvec + e] =
+        src ? src[static_cast<long long>(t) * nvec + e] : make_uint4(0u, 0u, 0u, 0u);
   }
 }
 
@@ -964,4 +1035,81 @@ extern "C" int yb_vae_frame_match(const void* kept, int t_kept, const void* x, i
   else YB_FM_LAUNCH(unsigned char);
 #undef YB_FM_LAUNCH
   return check_launch("vae_frame_match");
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Row-band forms (include/yume_b200_vae_rows.h)
+// ---------------------------------------------------------------------------------------------------------
+extern "C" int yb_vae_rms_act_rows(const void* x, long long ldx, void* out, void* send, const void* gamma, int T, int Hs, int Ws,
+                                   int C, int Cp, int up, int silu, void* stream_) {
+  if (!x || !out || T <= 0 || Hs <= 0 || Ws <= 0 || C <= 0) return YB_ERR_ARG;
+  if (C % 8 != 0 || Cp % 8 != 0 || Cp < C || (up != 1 && up != 2)) return YB_ERR_SHAPE;
+  if ((ldx % 8) || (reinterpret_cast<uintptr_t>(x) & 0xF) || (reinterpret_cast<uintptr_t>(out) & 0xF) ||
+      (reinterpret_cast<uintptr_t>(send) & 0xF))
+    return YB_ERR_ALIGNMENT;
+  if (C > 1024) return YB_ERR_SHAPE;
+  if (gamma && (reinterpret_cast<uintptr_t>(gamma) & 0xF)) return YB_ERR_ALIGNMENT;
+  const long long nvox = static_cast<long long>(T) * (Hs * up + 2) * Ws * up;   // the buffer's voxels: 32-bit indices
+  if (nvox > 0x7fffffffLL - (1LL << 24)) return YB_ERR_SHAPE;
+  // the (NCH, G) instance and grid of yb_vae_rms_act for the same arguments
+  const int nch = C <= 256 ? 1 : (C <= 512 ? 2 : 4);
+  const int g = nch > 1 ? 32 : (Cp <= 64 ? 8 : (Cp <= 128 ? 16 : 32));
+  const int per_block = 8 * (4 / nch) * (32 / g);
+  long long blocks = (static_cast<long long>(T) * Hs * up * Ws * up + per_block - 1) / per_block;
+  if (blocks > static_cast<long long>(sm_count()) * 32) blocks = static_cast<long long>(sm_count()) * 32;
+  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
+#define YB_RMS_ROWS_LAUNCH(NCH, G)                                                                                         \
+  rms_act_kernel<NCH, G, true><<<static_cast<int>(blocks), 256, 0, st>>>(                                                  \
+      static_cast<const __nv_bfloat16*>(x), ldx, static_cast<__nv_bfloat16*>(out), static_cast<const float*>(gamma), T, Hs, \
+      Ws, C, Cp, up, silu, static_cast<__nv_bfloat16*>(send))
+  if (nch == 4) YB_RMS_ROWS_LAUNCH(4, 32);
+  else if (nch == 2) YB_RMS_ROWS_LAUNCH(2, 32);
+  else if (g == 32) YB_RMS_ROWS_LAUNCH(1, 32);
+  else if (g == 16) YB_RMS_ROWS_LAUNCH(1, 16);
+  else YB_RMS_ROWS_LAUNCH(1, 8);
+#undef YB_RMS_ROWS_LAUNCH
+  return check_launch("vae_rms_act_rows");
+}
+
+static int rows_glue_check(const void* a, const void* b, const void* c, int T, int Hs, long long row_bytes) {
+  if (T <= 0 || Hs <= 0 || row_bytes <= 0) return YB_ERR_ARG;
+  if ((row_bytes % 16) || (reinterpret_cast<uintptr_t>(a) & 0xF) || (reinterpret_cast<uintptr_t>(b) & 0xF) ||
+      (reinterpret_cast<uintptr_t>(c) & 0xF))
+    return YB_ERR_ALIGNMENT;
+  return YB_OK;
+}
+
+extern "C" int yb_vae_rows_pack(const void* buf, void* send, int T, int Hs, long long row_bytes, void* stream_) {
+  if (!buf || !send) return YB_ERR_ARG;
+  if (int rc = rows_glue_check(buf, send, nullptr, T, Hs, row_bytes)) return rc;
+  rows_pack_kernel<<<grid_for(2LL * T * (row_bytes / 16)), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const uint4*>(buf), static_cast<uint4*>(send), T, Hs, row_bytes / 16);
+  return check_launch("vae_rows_pack");
+}
+
+extern "C" int yb_vae_rows_unpack(const void* recv_top, const void* recv_bot, void* buf, int T, int Hs, long long row_bytes,
+                                  void* stream_) {
+  if (!buf) return YB_ERR_ARG;
+  if (int rc = rows_glue_check(recv_top, recv_bot, buf, T, Hs, row_bytes)) return rc;
+  rows_unpack_kernel<<<grid_for(2LL * T * (row_bytes / 16)), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const uint4*>(recv_top), static_cast<const uint4*>(recv_bot), static_cast<uint4*>(buf), T, Hs, row_bytes / 16);
+  return check_launch("vae_rows_unpack");
+}
+
+extern "C" int yb_vae_unpatchify2_clamp_rows(const void* y, long long ldy, void* out, long long plane, long long frame, int T,
+                                             int Hs, int W, void* stream_) {
+  if (!y || !out || T <= 0 || Hs <= 0 || W <= 0 || ldy < 12 || frame < 4LL * Hs * W || plane < frame * T) return YB_ERR_ARG;
+  unpatchify2_clamp_rows_kernel<<<grid_for(12LL * T * Hs * W), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const float*>(y), ldy, static_cast<float*>(out), T, Hs, W, plane, frame);
+  return check_launch("vae_unpatchify2_clamp_rows");
+}
+
+extern "C" int yb_nhwc_to_nchw_f32_clamp_rows(const void* x, long long ldx, void* out, long long plane, long long frame, int T,
+                                              int Hs, int W, int Cn, float lo, float hi, void* stream_) {
+  if (!x || !out || T <= 0 || Hs <= 0 || W <= 0 || Cn <= 0 || ldx < Cn || frame < static_cast<long long>(Hs) * W ||
+      plane < frame * T || !(lo <= hi))
+    return YB_ERR_ARG;
+  nhwc_to_nchw_rows_kernel<<<grid_for(static_cast<long long>(T) * Hs * W * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      static_cast<const float*>(x), ldx, static_cast<float*>(out), T, Hs, W, Cn, lo, hi, plane, frame);
+  return check_launch("nhwc_to_nchw_clamp_rows");
 }

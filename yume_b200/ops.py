@@ -1093,3 +1093,112 @@ def conv3d_fp8(x: torch.Tensor, x_scale: torch.Tensor, w: torch.Tensor, w_scale:
     _launches += 1
     _flops += 2.0 * T * H * W * kt * kh * kw * Cp * w.shape[0]
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------
+# Row-band forms of the Wan VAE decode (include/yume_b200_vae_rows.h)
+# ------------------------------------------------------------------------------------------------------------
+def conv3d_rows(xbuf: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, T: int, H: int, W: int,
+                t_hist: int = 0, epilogue: int = YB_EPI_BF16, res: Optional[torch.Tensor] = None, taps=(3, 3, 3),
+                full_h: Optional[int] = None) -> torch.Tensor:
+    """Row-halo conv: xbuf bf16 [t_hist + T, H + 2, W, Cp] is a band buffer (rows 0 and H + 1 the neighbours' halo rows, or
+    zeros at the image's edge) -> out rows (t * H + h) * W + w of the band's H rows; t_hist 0 (causal zero padding in time) or
+    kt - 1 carried frames in front. full_h: the image's height; the launch then sums the kw taps the way the full-height launch
+    of T frames does (fused or not, yb_conv3d_plan), so its rows are that launch's bits."""
+    if taps[1] != 3:
+        raise YumeB200Error("conv3d_rows needs kh = 3")
+    fuse_w = 0
+    if full_h is not None:
+        plan = (C.c_int * 4)()
+        check(_lib.load().yb_conv3d_plan(T, full_h, W, w.shape[0], taps[2], 0, plan), "yb_conv3d_plan")
+        fuse_w = 2 if plan[3] else 1
+    args = _conv_args(xbuf, w, bias, out, (t_hist + T, H + 2, W), T, H, W, epilogue, res, taps, True, 1, 0, fuse_w, None, 1, 1)
+    check(_lib.load().yb_conv3d_rows(C.byref(args), t_hist, _stream()), "yb_conv3d_rows")
+    _count_conv(T, H, W, taps, 1, 1, xbuf.shape[-1], w.shape[0])
+    return out
+
+
+def vae_rms_act_rows(x: torch.Tensor, dims, out: torch.Tensor, gamma: Optional[torch.Tensor], up: int = 1, silu: bool = True,
+                     send: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x bf16 [T*Hs*Ws, C] -> rows 1 .. Hs*up of out bf16 [T, Hs*up + 2, Ws*up, Cp] (a band buffer's T new frames); send bf16
+    [2, T, Ws*up, Cp] (optional) gets the first and the last written row of every frame."""
+    global _launches
+    _need(x, torch.bfloat16, "x")
+    _need(out, torch.bfloat16, "out")
+    T, Hs, Ws = dims
+    if not out.is_contiguous() or tuple(out.shape[:3]) != (T, Hs * up + 2, Ws * up):
+        raise YumeB200Error(f"vae_rms_act_rows: out must be a contiguous [{T}, {Hs * up + 2}, {Ws * up}, Cp]")
+    if send is not None:
+        _need(send, torch.bfloat16, "send")
+        if not send.is_contiguous() or tuple(send.shape) != (2, T, Ws * up, out.shape[-1]):
+            raise YumeB200Error(f"vae_rms_act_rows: send must be a contiguous [2, {T}, {Ws * up}, {out.shape[-1]}]")
+    check(_lib.load().yb_vae_rms_act_rows(x.data_ptr(), x.stride(0), out.data_ptr(), _ptr(send), _ptr(gamma), T, Hs, Ws,
+                                          x.shape[1], out.shape[-1], up, 1 if silu else 0, _stream()), "yb_vae_rms_act_rows")
+    _launches += 1
+    return out
+
+
+def _band_frames(buf: torch.Tensor, name: str):
+    if buf.dtype != torch.bfloat16 or not buf.is_cuda or not buf.is_contiguous() or buf.dim() != 4:
+        raise YumeB200Error(f"{name}: the band buffer must be a contiguous CUDA bf16 [T, Hs + 2, W, Cp]")
+    return buf.shape[0], buf.shape[1] - 2, buf.shape[2] * buf.shape[3] * 2
+
+
+def vae_rows_pack(buf: torch.Tensor, send: torch.Tensor) -> torch.Tensor:
+    """send [2, T, W, Cp] = rows 1 and Hs of the band buffer frames buf [T, Hs + 2, W, Cp]."""
+    global _launches
+    T, Hs, row_bytes = _band_frames(buf, "vae_rows_pack")
+    if not send.is_contiguous() or send.dtype != buf.dtype or tuple(send.shape) != (2, T) + tuple(buf.shape[2:]):
+        raise YumeB200Error("vae_rows_pack: send must be a contiguous [2, T, W, Cp] of the buffer's dtype")
+    check(_lib.load().yb_vae_rows_pack(buf.data_ptr(), send.data_ptr(), T, Hs, row_bytes, _stream()), "yb_vae_rows_pack")
+    _launches += 1
+    return send
+
+
+def vae_rows_unpack(top: Optional[torch.Tensor], bot: Optional[torch.Tensor], buf: torch.Tensor) -> torch.Tensor:
+    """Rows 0 and Hs + 1 of the band buffer frames buf [T, Hs + 2, W, Cp] = top / bot [T, W, Cp] (zeros for None)."""
+    global _launches
+    T, Hs, row_bytes = _band_frames(buf, "vae_rows_unpack")
+    for t in (top, bot):
+        if t is not None and (not t.is_contiguous() or t.dtype != buf.dtype or tuple(t.shape) != (T,) + tuple(buf.shape[2:])):
+            raise YumeB200Error("vae_rows_unpack: halo rows must be contiguous [T, W, Cp] of the buffer's dtype")
+    check(_lib.load().yb_vae_rows_unpack(_ptr(top), _ptr(bot), buf.data_ptr(), T, Hs, row_bytes, _stream()),
+          "yb_vae_rows_unpack")
+    _launches += 1
+    return buf
+
+
+def _band_window(out: torch.Tensor, Cn: int, T: int, rows: int, cols: int, name: str):
+    """(plane, frame) strides of out = video[:, t0:t0 + T, r0:r0 + rows] (f32 view of a contiguous [Cn, F, H, cols] video)."""
+    _need(out, torch.float32, name)
+    c, t, h, w = out.shape
+    if (c, t, h, w) != (Cn, T, rows, cols) or out.stride(3) != 1 or out.stride(2) != w or out.stride(1) < h * w:
+        raise YumeB200Error(f"{name}: out must be a row band [{Cn}, {T}, {rows}, {cols}] of a contiguous video")
+    return out.stride(0), out.stride(1)
+
+
+def vae_unpatchify2_clamp_rows(y: torch.Tensor, out: torch.Tensor, T: int, Hs: int, W: int) -> torch.Tensor:
+    """vae_unpatchify2_clamp of a band into out = video[:, t0:t0 + T, 2 r0:2 (r0 + Hs)] (f32 [3, T, 2Hs, 2W] view)."""
+    global _launches
+    _need(y, torch.float32, "y")
+    plane, frame = _band_window(out, 3, T, 2 * Hs, 2 * W, "vae_unpatchify2_clamp_rows")
+    check(_lib.load().yb_vae_unpatchify2_clamp_rows(y.data_ptr(), y.stride(0), out.data_ptr(), plane, frame, T, Hs, W,
+                                                    _stream()), "yb_vae_unpatchify2_clamp_rows")
+    _launches += 1
+    return out
+
+
+def nhwc_to_nchw_f32_rows(x: torch.Tensor, out: torch.Tensor, clamp: Optional[tuple] = None) -> torch.Tensor:
+    """nhwc_to_nchw_f32 (optionally clamped) of a band into out = video[:, t0:t0 + T, r0:r0 + Hs] (f32 [Cn, T, Hs, W] view);
+    x f32 [T*Hs*W, ldx]."""
+    global _launches
+    _need(x, torch.float32, "x")
+    Cn, T, Hs, W = out.shape
+    plane, frame = _band_window(out, Cn, T, Hs, W, "nhwc_to_nchw_f32_rows")
+    if x.shape[0] != T * Hs * W:
+        raise YumeB200Error("nhwc_to_nchw_f32_rows: x rows must be the band's voxels")
+    lo, hi = (-math.inf, math.inf) if clamp is None else clamp
+    check(_lib.load().yb_nhwc_to_nchw_f32_clamp_rows(x.data_ptr(), x.stride(0), out.data_ptr(), plane, frame, T, Hs, W, Cn,
+                                                     float(lo), float(hi), _stream()), "yb_nhwc_to_nchw_f32_clamp_rows")
+    _launches += 1
+    return out

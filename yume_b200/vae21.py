@@ -95,7 +95,11 @@ class Wan21VaeDecoder(WanVaeDecoder):
         super().__init__(sd, z_dim, layers, mean, std, device, precision, resume)
 
     def _write(self, y: Tensor, out: Tensor, dims) -> None:
-        if self._one_pass:
+        if self._rows is not None:
+            _, hs, _ = dims
+            r = self._row0(hs)
+            ops.nhwc_to_nchw_f32_rows(y, out[:, :, r:r + hs], (-1.0, 1.0))
+        elif self._one_pass:
             ops.nhwc_to_nchw_f32(y, out.view(3, -1), clamp=(-1.0, 1.0))
         else:
             ops.nhwc_to_nchw_f32_win(y, out, (-1.0, 1.0))

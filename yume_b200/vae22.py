@@ -35,7 +35,8 @@ import torch
 from . import ops
 from ._lib import YumeB200Error
 from .dit import quantize_weight_fp8
-from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _rup, chunk_lengths  # noqa: F401  (chunk_lengths: re-exported)
+from .vae_rows import RowGroup
+from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _frames_of, _rup, chunk_lengths  # noqa: F401  (chunk_lengths: re-exported)
 
 Tensor = torch.Tensor
 
@@ -108,16 +109,41 @@ class WanVaeDecoder(WanVaeEngine):
         b[:zd] = W2 @ mean + sd["conv2.bias"].detach().float()
         self.lin["conv2"] = (w.to(dev, _BF16).contiguous(), b.to(dev))
 
+    def enable_row_parallel(self, group=None) -> "WanVaeDecoder":
+        """Decode on the ranks of `group` (torch.distributed; default the world), each rank its band of rows: rank r of P owns
+        latent rows [floor(rH/P), floor((r+1)H/P)) and every level's rows above them. Every rank still passes the full latent and
+        gets the full clamped video, equal bit for bit to the one-GPU decode: the convs read one halo row of each neighbouring
+        band (exchanged after every norm pass), the mid attention runs on the gathered full frames, and one all-gather at the end
+        of a call assembles the video. A group of one rank keeps the one-GPU path. Call it on every rank; every later decode
+        is then a collective of the group. Raises YumeB200Error without an initialised process group or with precision="fp8"."""
+        if self.precision == "fp8":
+            raise YumeB200Error("enable_row_parallel: the fp8 decode has no row-parallel form; use precision='bf16'")
+        rows = RowGroup(group)
+        self._rows = rows if rows.world > 1 else None
+        self.reset()                                             # kept carries would belong to another band
+        return self
+
     def _input(self, L: Layer, z: Tensor):
-        """conv2 (latent de-normalisation folded in) and decoder.conv1 on one chunk of the latent."""
+        """conv2 (latent de-normalisation folded in) and decoder.conv1 on one chunk of the latent (this rank's band of its rows
+        under a row-parallel decode)."""
         zd, T, H, W = z.shape
+        if self._rows is not None:
+            r0, hs, _ = self._band
+            z, H = z[:, :, r0:r0 + hs], hs
         N = T * H * W
         zl = self._new(N, 64)
         ops.nchw_to_nhwc_bf16(z.to(self.device, _F32).reshape(zd, N).contiguous(), zl)
         w2, b2 = self.lin["conv2"]
+        dims = (T, H, W)
+        if self._rows is not None:                               # conv1's band buffer: each frame's rows, then the halo rows
+            x0 = self._hist_buf(L.name, T, H, W, 64, zero=True, halo=True)
+            h = x0.shape[0] - T
+            for t in range(T):
+                ops.gemm(zl[t * H * W:(t + 1) * H * W], w2, b2, x0[h + t, 1:H + 1].view(-1, 64)[:, :w2.shape[0]], ops.YB_EPI_BF16)
+            self._halo(x0, T)
+            return self._conv(L.name, x0, dims, key=L.name), dims
         x0 = self._hist_buf(L.name, T, H, W, 64, zero=True)
         ops.gemm(zl, w2, b2, x0.view(-1, 64)[x0.shape[0] * H * W - N:, :w2.shape[0]], ops.YB_EPI_BF16)
-        dims = (T, H, W)
         return self._conv(L.name, x0, dims, key=L.name), dims
 
     def _resample(self, L: Layer, x: Tensor, dims):
@@ -149,12 +175,35 @@ class WanVaeDecoder(WanVaeEngine):
                 x, T = y, y.shape[0] // HW
             else:
                 self._keep(key, self._new(0, H, W, _rup(C, 64)))
-        a = self._act(x, (T, H, W), None, False, up=2, conv=p + ".resample.1")   # nearest-exact 2x, then Conv2d 3x3 (zero pad 1)
+        a = self._act(x, (T, H, W), None, False, up=2, conv=p + ".resample.1", halo=True)  # nearest-exact 2x, then Conv2d 3x3
         return self._conv(p + ".resample.1", a, (T, 2 * H, 2 * W)), (T, 2 * H, 2 * W)
 
     def _head(self, L: Layer, x: Tensor, dims, out: Tensor) -> None:
-        y = self._conv(L.name, self._act(x, dims, "decoder.head.0", True, key=L.name), dims, epilogue=ops.YB_EPI_F32, key=L.name)
+        y = self._conv(L.name, self._act(x, dims, "decoder.head.0", True, key=L.name, halo=True), dims, epilogue=ops.YB_EPI_F32,
+                       key=L.name)
         self._write(y, out, dims)
+
+    def _row0(self, rows: int) -> int:
+        """First row of this rank's band at a level whose band has `rows` rows."""
+        r0, hs, _ = self._band
+        return r0 * (rows // hs)
+
+    def _stream(self, src: Tensor, out: Tensor, lengths: Sequence[int], k_in: int, k_out: int, u0: int = 0, *args, **kw):
+        """WanVaeEngine._stream; a row-parallel decode then all-gathers the bands of the frames it wrote."""
+        res = super()._stream(src, out, lengths, k_in, k_out, u0, *args, **kw)
+        t0 = _frames_of(u0, k_out)
+        if self._rows is not None and t0 < out.shape[1]:
+            _, _, H = self._band
+            S = out.shape[2] // H
+            r0, hs, _ = self._band
+            mine = out[:, t0:, r0 * S:(r0 + hs) * S]
+            sizes = [S * h for h in self._rows.sizes(H)]
+            row = 0
+            for r, b in enumerate(self._rows.gather(mine, 2, sizes)):
+                if r != self._rows.rank:
+                    out[:, t0:, row:row + sizes[r]].copy_(b)
+                row += sizes[r]
+        return res
 
     def _t_scale(self) -> int:
         return math.prod(L.ft for L in self.layers if L.kind == "up")
@@ -168,6 +217,12 @@ class WanVaeDecoder(WanVaeEngine):
         memory. With resume=True a latent that extends the last call's latent runs only its new frames (WanVaeEngine._resumed)."""
         if z.dim() != 4 or z.shape[0] != self.z_dim:
             raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
+        if self._rows is not None:                               # checked on every rank before the first collective
+            H, P = z.shape[2], self._rows.world
+            if H < P:
+                raise YumeB200Error(f"a row-parallel decode on {P} ranks needs at least {P} latent rows, got {H}")
+            r0, r1 = self._rows.band(H)
+            self._band = (r0, r1 - r0, H)
         if self.resume:
             T, H, W = z.shape[1:]
             src = z.to(self.device, _F32).contiguous()
@@ -236,7 +291,11 @@ class Wan22VaeDecoder(WanVaeDecoder):
                 del self.conv[name]                              # no bf16 copy of a converted weight is kept
 
     def _write(self, y: Tensor, out: Tensor, dims) -> None:
-        if self._one_pass:
+        if self._rows is not None:
+            T, hs, W = dims
+            r = 2 * self._row0(hs)
+            ops.vae_unpatchify2_clamp_rows(y, out[:, :, r:r + 2 * hs], T, hs, W)
+        elif self._one_pass:
             ops.vae_unpatchify2_clamp(y, out, *dims)
         else:
             ops.vae_unpatchify2_clamp_win(y, out, *dims)

@@ -56,6 +56,11 @@ class WanVaeEngine:
     # s_w f32 [cop], bias f32 [cop], taps). Their input streams are (e4m3 frames, scale frames) pairs, see _hist_buf.
     conv8: Dict[str, Tuple[Tensor, Tensor, Tensor, tuple]] = {}
     _kept: Optional[_Kept] = None   # resume=True: the state kept from the last call
+    # row-parallel decode (WanVaeDecoder.enable_row_parallel): the RowGroup of the ranks (None: one rank decodes everything) and,
+    # during a call, the band (r0, rows, H) of the latent's H rows this rank owns. dims are then the band's (T, rows, W), and the
+    # input of every conv with kh = 3 is a band buffer with one halo row above and below (include/yume_b200_vae_rows.h).
+    _rows = None
+    _band: Tuple[int, int, int] = (0, 0, 0)
 
     def __init__(self, sd: Dict[str, Tensor], z_dim: int, layers: List[Layer], mean: Optional[Tensor], std: Optional[Tensor],
                  device, precision: str = "bf16", resume: bool = False):
@@ -138,11 +143,14 @@ class WanVaeEngine:
         """The running chunk is the whole sequence: it issues the one-pass launches."""
         return self._chunk == 0 and not self._more
 
-    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0, fp8: bool = False):
+    def _hist_buf(self, key: Optional[str], T: int, H: int, W: int, Cp: int, zero: bool = False, n: int = 0, fp8: bool = False,
+                  halo: bool = False):
         """Input buffer [h + T, H, W, Cp] of a conv whose input stream is `key`: after the first chunk its first h frames (n, or
         HIST when n is 0) are the frames carried from the previous chunk and the producer writes the T new frames behind them.
-        fp8: the pair (e4m3 [h + T, H, W, Cp], f32 scales [h + T, Cp / 128, H, W]) of an e4m3 conv's input, frames carried alike."""
+        fp8: the pair (e4m3 [h + T, H, W, Cp], f32 scales [h + T, Cp / 128, H, W]) of an e4m3 conv's input, frames carried alike.
+        halo: a band buffer [h + T, H + 2, W, Cp] (carried frames with their halo rows)."""
         h = (n or self.HIST) if (key is not None and self._chunk > 0) else 0
+        H = H + 2 if halo else H
         if fp8:
             buf = (self._new(h + T, H, W, Cp, dtype=_E4M3), self._new(h + T, Cp // 128, H, W, dtype=_F32))
             if h:
@@ -191,7 +199,9 @@ class WanVaeEngine:
         if out is None:
             To, Ho, Wo = ops.conv_out_dims(T, H, W, taps, stride_t, stride_hw)
             out = self._new(To * Ho * Wo, w.shape[0], dtype=_F32 if epilogue == ops.YB_EPI_F32 else _BF16)
-        if h:
+        if self._rows is not None and a.shape[1] == H + 2:       # a band buffer (_act with halo): the row-halo conv
+            ops.conv3d_rows(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, full_h=self._band[2] * (H // self._band[1]))
+        elif h:
             ops.conv3d_causal_hist(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, out_t_mul=out_t_mul,
                                    out_t_add=out_t_add, stride_t=stride_t, stride_hw=stride_hw)
         else:
@@ -200,12 +210,19 @@ class WanVaeEngine:
         return out
 
     def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1, key: Optional[str] = None,
-             n: int = 0, conv: Optional[str] = None):
+             n: int = 0, conv: Optional[str] = None, halo: bool = False):
         """The input buffer of the conv `conv` (see _hist_buf): RMS_norm * gamma, SiLU, 2x upsample of x; an e4m3 pair when that
-        conv is one of conv8."""
+        conv is one of conv8. halo (a conv with kh = 3) under a row-parallel decode: a band buffer whose halo rows of the T new
+        frames come from the neighbouring ranks."""
         ops = self.ops
         T, H, W = dims
         g = self.gamma[gamma] if gamma else None
+        if halo and self._rows is not None:
+            out = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n, halo=True)
+            send = self._new(2, T, W * up, out.shape[-1])
+            ops.vae_rms_act_rows(x, dims, out[out.shape[0] - T:], g, up, silu, send=send)
+            self._halo(out, T, send)
+            return out
         if conv in self.conv8:
             q, s = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n, fp8=True)
             ops.vae_rms_act_fp8(x, dims, q[q.shape[0] - T:], s[s.shape[0] - T:], g, up, silu)
@@ -214,17 +231,37 @@ class WanVaeEngine:
         ops.vae_rms_act(x, dims, out[out.shape[0] - T:], g, up, silu)
         return out
 
+    def _halo(self, buf: Tensor, T: int, send: Optional[Tensor] = None) -> None:
+        """Fill the halo rows of the T new frames of the band buffer `buf` from the neighbouring ranks (zeros at the image's
+        edge). send [2, T, W, Cp]: the band's top and bottom rows of those frames, packed from `buf` when not given."""
+        new = buf[buf.shape[0] - T:]
+        if send is None:
+            send = self._new(2, T, *buf.shape[2:])
+            self.ops.vae_rows_pack(new, send)
+        top, bot = self._rows.exchange(send)
+        self.ops.vae_rows_unpack(top, bot, new)
+
+    def _attention_rows(self, p: str, x: Tensor, dims) -> Tensor:
+        """The mid attention of a row-parallel decode: every rank gathers the full frames, runs `_attention` on them (the same
+        launches as one rank) and keeps its own rows."""
+        T, hs, W = dims
+        r0, _, H = self._band
+        C = x.shape[1]
+        full = torch.cat(self._rows.gather(x.view(T, hs, W, C), 1, self._rows.sizes(H)), 1)
+        y = self._attention(p, full.view(T * H * W, C), (T, H, W))
+        return y.view(T, H, W, C)[:, r0:r0 + hs].reshape(T * hs * W, C)
+
     def _res_block(self, p: str, x: Tensor, dims) -> Tensor:
         """ResidualBlock (vae2_2.py:195-239)."""
         ops = self.ops
         c1, c2 = p + ".residual.2", p + ".residual.6"
-        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1, conv=c1), dims, key=c1)
+        y = self._conv(c1, self._act(x, dims, p + ".residual.0", True, key=c1, conv=c1, halo=True), dims, key=c1)
         res = x
         if (p + ".shortcut") in self.lin:
             w, b = self.lin[p + ".shortcut"]
             res = self._new(x.shape[0], w.shape[0])
             ops.gemm(x, w, b, res, ops.YB_EPI_BF16)
-        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2, conv=c2), dims, res=res, key=c2)
+        return self._conv(c2, self._act(y, dims, p + ".residual.3", True, key=c2, conv=c2, halo=True), dims, res=res, key=c2)
 
     def _attention(self, p: str, x: Tensor, dims) -> Tensor:
         """AttentionBlock (vae2_2.py:242-283): per-frame single-head attention over H*W tokens, d = C."""
@@ -277,7 +314,7 @@ class WanVaeEngine:
             elif L.kind == "res":
                 x = self._res_block(L.name, x, dims)
             elif L.kind == "attn":
-                x = self._attention(L.name, x, dims)
+                x = self._attention(L.name, x, dims) if self._rows is None else self._attention_rows(L.name, x, dims)
             elif L.kind == "hold":
                 held, held_dims = x, dims
             elif L.kind in ("up", "down"):
@@ -358,6 +395,8 @@ class WanVaeEngine:
         match = torch.empty(2, dtype=torch.int32, device=self.device)
         self.ops.vae_frame_match(kept.src if comparable else None, src, match)
         first, zero = match.tolist()                             # the one synchronisation a resuming call adds
+        if self._rows is not None:                               # every rank resumes from the same snapshot
+            first = self._rows.min_int(first if comparable else 0)
         snaps = kept.snaps if comparable else {}
         P = max((p for p in snaps if p <= first), default=0)
         u0, carry = snaps[P] if P else (0, None)
@@ -383,6 +422,22 @@ class WanVaeEngine:
 
     # ---- chunk planner -------------------------------------------------------------------------------------
     def chunk_bytes(self, n: int, T: int, H: int, W: int) -> int:
+        """`_chunk_bytes`, or under a row-parallel decode the bound of one rank (`_band_bytes`)."""
+        return self._chunk_bytes(n, T, H, W) if self._rows is None else self._band_bytes(n, T, H, W)
+
+    def _band_bytes(self, n: int, T: int, H: int, W: int) -> int:
+        """Upper bound of one rank's device bytes in a row-parallel decode: the largest band, its halo rows counted at every level
+        as two more latent rows, plus the gathered attention input (padded bands, full frames, the attention's own buffers and
+        the rows kept), and the whole video with the padded bands of its all-gather."""
+        P = self._rows.world
+        hb = -(-H // P)
+        attn = next(L for L in self.layers if L.kind == "attn")
+        s = next(L for L in self.layers if L.kind == "in").ft
+        F, c = n * s, attn.ci
+        gathered = ((P + 2) * F * hb * W + F * H * W) * c * 2 + _attn_bytes(F, H * W, c)
+        return self._chunk_bytes(n, T, hb + 2, W) + gathered + (1 + P) * self._fixed_bytes(T, H, W)
+
+    def _chunk_bytes(self, n: int, T: int, H: int, W: int) -> int:
         """Upper bound of the device bytes a decode (encode) of T latent (video) frames at H x W allocates on top of the weights
         and its input when its chunks hold n latent frames: the whole result, every carried history, and the largest set of
         activations one step of the layer list keeps live (every buffer of that step counted as live at once; a chunk after
@@ -413,8 +468,7 @@ class WanVaeEngine:
                 carries += hist * vox * (cp + _rup(co, 64)) * bf
                 live = F * vox * (2 * c + 3 * co) * bf + (F + hist) * vox * (cp + _rup(co, 64)) * bf
             elif L.kind == "attn":
-                Lf, Next = _rup(vox, 32), _rup(F * vox, 32) + 32
-                live = (F * vox * c * 5 + Next * c * 3 + F * Lf * c * 3) * bf + vox * Lf * (f4 + bf)
+                live = _attn_bytes(F, vox, c)
             elif L.kind == "up":
                 t_up = L.ft == 2
                 F2 = 2 * F if t_up else F
@@ -435,12 +489,28 @@ class WanVaeEngine:
         """Latent frames per chunk: all `units` when they fit (and always off CUDA), else the longest chunks whose `nbytes`
         fit the device's free memory (free + torch's cached, unallocated blocks) minus MEM_MARGIN. The free memory is read
         when the call starts, so other work on the same GPU can make a sequence that would fit alone run in chunks (with the
-        same result)."""
+        same result). A row-parallel decode plans with the smallest budget of its ranks, so that all run the same chunks."""
+        free = self._free_bytes()
+        budget = _UNBOUNDED if free is None else free - self.MEM_MARGIN
+        if self._rows is not None:
+            budget = self._rows.min_int(budget)
+        return [units] if budget == _UNBOUNDED else chunk_lengths(units, nbytes, budget)
+
+    def _free_bytes(self) -> Optional[int]:
+        """Free device memory the planner may use (free + torch's cached, unallocated blocks); None off CUDA."""
         if self.device.type != "cuda":
-            return [units]
+            return None
         free, _ = torch.cuda.mem_get_info(self.device)
-        free += torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
-        return chunk_lengths(units, nbytes, free - self.MEM_MARGIN)
+        return free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+
+
+_UNBOUNDED = 1 << 62                # the planner's budget off CUDA: everything in one chunk
+
+
+def _attn_bytes(F: int, vox: int, c: int) -> int:
+    """Bytes the mid attention (`_attention`) allocates for F frames of vox tokens and c channels."""
+    Lf, Next = _rup(vox, 32), _rup(F * vox, 32) + 32
+    return (F * vox * c * 5 + Next * c * 3 + F * Lf * c * 3) * 2 + vox * Lf * (4 + 2)
 
 
 def chunk_lengths(T: int, nbytes, budget: int) -> List[int]:
