@@ -191,6 +191,13 @@ ROWS_SIGNATURES = {
     "yb_nhwc_to_nchw_f32_clamp_rows": (_i, [_vp, _ll, _vp, _ll, _ll, _i, _i, _i, _i, _f, _f, _vp]),
 }
 
+# every symbol include/yume_b200_vae_rows_enc.h declares (the row-band forms of a row-parallel Wan VAE encode)
+ROWS_ENC_SIGNATURES = {
+    "yb_conv3d_rows_down": (_i, [C.POINTER(Conv3dArgs), _vp]),
+    "yb_vae_patchify2_bf16_rows": (_i, [_vp, _ll, _vp, _i, _i, _i, _i, _i, _i, _vp]),
+    "yb_nchw_to_nhwc_bf16_rows": (_i, [_vp, _ll, _vp, _i, _i, _i, _i, _i, _i, _i, _vp]),
+}
+
 _lib = None
 
 
@@ -213,7 +220,7 @@ def load():
                             "(python -m yume_b200.build --force)")
     for name, (res, args) in {**SIGNATURES, **CLIP_SIGNATURES, **T5_SIGNATURES, **STREAM_SIGNATURES,
                               **FP8_SIGNATURES, **FP8_ATTN_SIGNATURES, **FP8_VAE_SIGNATURES, **RESUME_SIGNATURES,
-                              **FP8_SP_SIGNATURES, **ROWS_SIGNATURES}.items():
+                              **FP8_SP_SIGNATURES, **ROWS_SIGNATURES, **ROWS_ENC_SIGNATURES}.items():
         fn = getattr(lib, name)  # AttributeError here means header and library disagree
         fn.restype = res
         fn.argtypes = args

@@ -21,7 +21,8 @@ HEADERS = ["yb_ptx.cuh", "yb_host.h", "../../include/yume_b200.h", "../../includ
            "../../include/yume_b200_t5.h", "../../include/yume_b200_stream.h",
            "../../include/yume_b200_fp8.h", "../../include/yume_b200_fp8_attn.h",
            "../../include/yume_b200_fp8_vae.h", "../../include/yume_b200_vae_resume.h",
-           "../../include/yume_b200_fp8_sp.h", "../../include/yume_b200_vae_rows.h"]
+           "../../include/yume_b200_fp8_sp.h", "../../include/yume_b200_vae_rows.h",
+           "../../include/yume_b200_vae_rows_enc.h"]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

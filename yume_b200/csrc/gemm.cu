@@ -29,6 +29,7 @@
 #include "yb_host.h"
 #include "../../include/yume_b200_stream.h"
 #include "../../include/yume_b200_vae_rows.h"
+#include "../../include/yume_b200_vae_rows_enc.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -1011,7 +1012,11 @@ extern "C" int yb_gemm_bf16(const yb_gemm_args* a, void* stream_) {
 // and those frames take the place of the causal zero padding in time (the tensor map spans all t_hist + T frames).
 // rows is the row-halo form (include/yume_b200_vae_rows.h): the input has H + 2 rows, the two outer ones the neighbours' halo
 // rows, and output row h reads input rows h .. h + 2 (no zero fill in H; the tile plan is the one of the H output rows).
-static int conv3d_launch(const yb_conv3d_args* a, int t_hist, bool rows, void* stream_) {
+// down is its strided form (include/yume_b200_vae_rows_enc.h): the map starts at row 1 of the band buffer and spans H + 1 rows,
+// the last the halo row below, with the buffer's frame pitch; output row h reads map rows 2h .. 2h + 2 as the full-height map does.
+enum ConvRows { kConvFull = 0, kConvRows = 1, kConvRowsDown = 2 };
+static int conv3d_launch(const yb_conv3d_args* a, int t_hist, ConvRows form, void* stream_) {
+  const bool rows = form == kConvRows, down = form == kConvRowsDown;
   using namespace yb;
   if (!a || !a->xpad || !a->w || !a->out) return YB_ERR_ARG;
   if (a->struct_bytes != sizeof(yb_conv3d_args)) return YB_ERR_ARG;
@@ -1037,6 +1042,8 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, bool rows, void* s
   // history: exactly the kt-1 frames of the causal pad (unit stride), or the one frame the stride-2 time_conv carries
   if (t_hist > 0 && (!a->oob_zero_pad || t_hist != (st_t > 1 ? 1 : kt - 1))) return YB_ERR_ARG;
   if (rows && (!a->oob_zero_pad || strided || kh != 3)) return YB_ERR_ARG;
+  if (down && (!a->oob_zero_pad || st_hw != 2 || st_t != 1 || kt != 1 || kh != 3 || kw != 3 || t_hist || (a->H % 2)))
+    return YB_ERR_ARG;
   const int inT = a->T + t_hist;   // frames the tensor map spans
   int oT = a->T, oH = a->H, oW = a->W;
   if (st_t > 1) oT = (inT - kt) / st_t + 1;
@@ -1072,8 +1079,11 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, bool rows, void* s
   p.res_ld = a->res_ld;
   CUtensorMap tmA, tmB;
   const int padT = a->oob_zero_pad ? 0 : kt - 1, padH = a->oob_zero_pad ? 0 : kh - 1, padW = a->oob_zero_pad ? 0 : kw - 1;
-  int rc = make_tmap_bf16_4d(&tmA, a->xpad, inT + padT, a->H + (rows ? 2 : padH), a->W + padW, a->Cp, p.TT, p.TH,
-                             fuse_w ? CONVW_ROWS : p.TW, 64, st_t, st_hw, st_hw);
+  const uint64_t row_elems = static_cast<uint64_t>(a->W) * a->Cp;
+  int rc = down ? make_tmap_bf16_4d(&tmA, static_cast<const __nv_bfloat16*>(a->xpad) + row_elems, inT, a->H + 1, a->W, a->Cp,
+                                    p.TT, p.TH, p.TW, 64, st_t, st_hw, st_hw, (a->H + 2) * row_elems)
+                : make_tmap_bf16_4d(&tmA, a->xpad, inT + padT, a->H + (rows ? 2 : padH), a->W + padW, a->Cp, p.TT, p.TH,
+                                    fuse_w ? CONVW_ROWS : p.TW, 64, st_t, st_hw, st_hw);
   if (rc) return rc;
   rc = make_tmap_bf16_2d(&tmB, a->w, a->Cout, static_cast<uint64_t>(taps) * a->Cp, static_cast<uint64_t>(taps) * a->Cp,
                          block_n, GEMM_BLOCK_K);
@@ -1107,13 +1117,17 @@ static int conv3d_launch(const yb_conv3d_args* a, int t_hist, bool rows, void* s
 #undef YB_CONV_DISPATCH
 }
 
-extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream) { return conv3d_launch(a, 0, false, stream); }
+extern "C" int yb_conv3d_causal(const yb_conv3d_args* a, void* stream) { return conv3d_launch(a, 0, kConvFull, stream); }
 
 extern "C" int yb_conv3d_causal_hist(const yb_conv3d_args* a, int t_hist, void* stream) {
   if (t_hist <= 0) return YB_ERR_ARG;
-  return conv3d_launch(a, t_hist, false, stream);
+  return conv3d_launch(a, t_hist, kConvFull, stream);
 }
 
 extern "C" int yb_conv3d_rows(const yb_conv3d_args* a, int t_hist, void* stream) {
-  return conv3d_launch(a, t_hist, true, stream);
+  return conv3d_launch(a, t_hist, kConvRows, stream);
+}
+
+extern "C" int yb_conv3d_rows_down(const yb_conv3d_args* a, void* stream) {
+  return conv3d_launch(a, 0, kConvRowsDown, stream);
 }

@@ -11,6 +11,7 @@
 #include "../../include/yume_b200_fp8_vae.h"
 #include "../../include/yume_b200_vae_resume.h"
 #include "../../include/yume_b200_vae_rows.h"
+#include "../../include/yume_b200_vae_rows_enc.h"
 #include "yb_ptx.cuh"
 
 namespace yb {
@@ -718,6 +719,53 @@ __global__ void rows_unpack_kernel(const uint4* __restrict__ top, const uint4* _
   }
 }
 
+// Band readers of a row-parallel encode (include/yume_b200_vae_rows_enc.h): the T frames of a band buffer [T, hs + 2, Wo, ldo],
+// buffer row j = image row r0 - 1 + j of the level (zeros outside the image), each element converted as the _win readers do
+__global__ void patchify2_bf16_rows_kernel(const float* __restrict__ video, __nv_bfloat16* __restrict__ out, int ldo, int T,
+                                           int H, int W, long long plane, int r0, int hs) {
+  const int Hh = H / 2, Wh = W / 2;
+  const long long total = static_cast<long long>(T) * (hs + 2) * Wh;
+  for (long long v = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; v < total;
+       v += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int w = static_cast<int>(v % Wh);
+    const long long rr = v / Wh;
+    const int h = r0 - 1 + static_cast<int>(rr % (hs + 2));
+    const int f = static_cast<int>(rr / (hs + 2));
+    __nv_bfloat16* o = out + v * ldo;
+    int c0 = 0;
+    if (h >= 0 && h < Hh) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const float* src = video + c * plane + (static_cast<long long>(f) * H + 2 * h) * W + 2 * w;
+        const float2 top = *reinterpret_cast<const float2*>(src);
+        const float2 bot = *reinterpret_cast<const float2*>(src + W);
+        o[c * 4 + 0] = __float2bfloat16_rn(top.x);
+        o[c * 4 + 1] = __float2bfloat16_rn(bot.x);
+        o[c * 4 + 2] = __float2bfloat16_rn(top.y);
+        o[c * 4 + 3] = __float2bfloat16_rn(bot.y);
+      }
+      c0 = 12;
+    }
+    for (int c = c0; c < ldo; ++c) o[c] = __float2bfloat16_rn(0.0f);
+  }
+}
+
+__global__ void nchw_to_nhwc_rows_kernel(const float* __restrict__ x, __nv_bfloat16* __restrict__ out, int ldo, int T, int H,
+                                         int W, int Cn, long long plane, int r0, int hs) {
+  const long long total = static_cast<long long>(T) * (hs + 2) * W * ldo;
+  for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < total;
+       i += static_cast<long long>(gridDim.x) * blockDim.x) {
+    const int c = static_cast<int>(i % ldo);
+    const long long v = i / ldo;
+    const int w = static_cast<int>(v % W);
+    const long long rr = v / W;
+    const int h = r0 - 1 + static_cast<int>(rr % (hs + 2));
+    const int f = static_cast<int>(rr / (hs + 2));
+    out[i] = __float2bfloat16_rn(c < Cn && h >= 0 && h < H ? x[static_cast<long long>(c) * plane + (static_cast<long long>(f) * H + h) * W + w]
+                                                            : 0.f);
+  }
+}
+
 inline int grid_for(long long total) {
   long long b = (total + 255) / 256;
   const long long cap = static_cast<long long>(sm_count()) * 16;
@@ -1112,4 +1160,39 @@ extern "C" int yb_nhwc_to_nchw_f32_clamp_rows(const void* x, long long ldx, void
   nhwc_to_nchw_rows_kernel<<<grid_for(static_cast<long long>(T) * Hs * W * Cn), 256, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       static_cast<const float*>(x), ldx, static_cast<float*>(out), T, Hs, W, Cn, lo, hi, plane, frame);
   return check_launch("nhwc_to_nchw_clamp_rows");
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// Band readers of the row-parallel encode (include/yume_b200_vae_rows_enc.h)
+// ---------------------------------------------------------------------------------------------------------
+static int rows_reader_check(const void* src, long long plane, const void* out, int ldo, int T, int H, int W, int rows, int r0,
+                             int hs) {
+  if (!src || !out || T <= 0 || H <= 0 || W <= 0 || hs <= 0 || r0 < 0 || r0 + hs > rows) return YB_ERR_ARG;
+  if (plane < static_cast<long long>(T) * H * W) return YB_ERR_ARG;
+  if ((ldo % 8) || (reinterpret_cast<uintptr_t>(out) & 0xF)) return YB_ERR_ALIGNMENT;
+  return YB_OK;
+}
+
+extern "C" int yb_vae_patchify2_bf16_rows(const void* video, long long plane, void* out, int ldo, int T, int H, int W, int r0,
+                                          int hs, void* stream_) {
+  if (H <= 0 || W <= 0 || ldo < 12) return YB_ERR_ARG;
+  if ((H % 2) || (W % 2)) return YB_ERR_SHAPE;
+  if (int rc = rows_reader_check(video, plane, out, ldo, T, H, W, H / 2, r0, hs)) return rc;
+  if ((reinterpret_cast<uintptr_t>(video) & 0x7) || (plane % 2)) return YB_ERR_ALIGNMENT;
+  patchify2_bf16_rows_kernel<<<grid_for(static_cast<long long>(T) * (hs + 2) * (W / 2)), 256, 0,
+                               reinterpret_cast<cudaStream_t>(stream_)>>>(static_cast<const float*>(video),
+                                                                          static_cast<__nv_bfloat16*>(out), ldo, T, H, W, plane,
+                                                                          r0, hs);
+  return check_launch("vae_patchify2_bf16_rows");
+}
+
+extern "C" int yb_nchw_to_nhwc_bf16_rows(const void* x, long long plane, void* out, int ldo, int T, int H, int W, int Cn, int r0,
+                                         int hs, void* stream_) {
+  if (Cn <= 0 || ldo < Cn) return YB_ERR_ARG;
+  if (int rc = rows_reader_check(x, plane, out, ldo, T, H, W, H, r0, hs)) return rc;
+  nchw_to_nhwc_rows_kernel<<<grid_for(static_cast<long long>(T) * (hs + 2) * W * ldo), 256, 0,
+                             reinterpret_cast<cudaStream_t>(stream_)>>>(static_cast<const float*>(x),
+                                                                        static_cast<__nv_bfloat16*>(out), ldo, T, H, W, Cn, plane,
+                                                                        r0, hs);
+  return check_launch("nchw_to_nhwc_bf16_rows");
 }

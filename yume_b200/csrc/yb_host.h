@@ -112,16 +112,18 @@ inline int make_tmap_bf16_3d(CUtensorMap* tm, const void* base, uint64_t chunks,
   return r == CUDA_SUCCESS ? YB_OK : YB_ERR_TENSORMAP;
 }
 
-// 4D bf16 tensor map over a dense channels-last volume [T, H, W, C], box {bc, bw, bh, bt} (conv3d A operand).
+// 4D bf16 tensor map over a channels-last volume [T, H, W, C], box {bc, bw, bh, bt} (conv3d A operand). Frames are
+// `frame` elements apart, or H * W * C (dense) when it is 0.
 inline int make_tmap_bf16_4d(CUtensorMap* tm, const void* base, uint64_t T, uint64_t H, uint64_t W, uint64_t C,
                              uint32_t bt, uint32_t bh, uint32_t bw, uint32_t bc, uint32_t st = 1, uint32_t sh = 1,
-                             uint32_t sw = 1) {
+                             uint32_t sw = 1, uint64_t frame = 0) {
   // st/sh/sw > 1: the map samples every s-th voxel of that axis (elementStrides); a box of b OUTPUT voxels spans b*s input voxels
   PFN_encodeTiled fn = get_encode_fn();
   if (!fn) return YB_ERR_NO_DRIVER;
-  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || ((C * 2) & 0xF)) return YB_ERR_ALIGNMENT;
+  if (!frame) frame = H * W * C;
+  if ((reinterpret_cast<uintptr_t>(base) & 0xF) || ((C * 2) & 0xF) || ((frame * 2) & 0xF)) return YB_ERR_ALIGNMENT;
   cuuint64_t gdim[4] = {C, W, H, T};
-  cuuint64_t gstride[3] = {C * 2, W * C * 2, H * W * C * 2};
+  cuuint64_t gstride[3] = {C * 2, W * C * 2, frame * 2};
   cuuint32_t box[4] = {bc, bw * sw, bh * sh, bt * st};
   cuuint32_t estr[4] = {1, sw, sh, st};
   if (box[1] > 256 || box[2] > 256 || box[3] > 256) return YB_ERR_SHAPE;

@@ -1202,3 +1202,50 @@ def nhwc_to_nchw_f32_rows(x: torch.Tensor, out: torch.Tensor, clamp: Optional[tu
                                                      float(lo), float(hi), _stream()), "yb_nhwc_to_nchw_f32_clamp_rows")
     _launches += 1
     return out
+
+
+# ------------------------------------------------------------------------------------------------------------
+# Row-band forms of the Wan VAE encode (include/yume_b200_vae_rows_enc.h)
+# ------------------------------------------------------------------------------------------------------------
+def conv3d_rows_down(xbuf: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], out: torch.Tensor, T: int, H: int,
+                     W: int, epilogue: int = YB_EPI_BF16) -> torch.Tensor:
+    """Resample downsample2d of a band (ZeroPad2d((0,1,0,1)) + Conv2d 3x3 stride 2): xbuf bf16 [T, H + 2, W, Cp] a band buffer
+    of the band's H input rows, row H + 1 the first row of the band below (zeros on the last band), row 0 not read -> out rows
+    (t * H/2 + h) * W/2 + w, those rows of conv3d_causal(stride_hw=2) over the full-height input."""
+    args = _conv_args(xbuf, w, bias, out, (T, H + 2, W), T, H, W, epilogue, None, (1, 3, 3), True, 1, 0, 0, None, 1, 2)
+    check(_lib.load().yb_conv3d_rows_down(C.byref(args), _stream()), "yb_conv3d_rows_down")
+    _count_conv(T, H, W, (1, 3, 3), 1, 2, xbuf.shape[-1], w.shape[0])
+    return out
+
+
+def _rows_reader(src: torch.Tensor, out: torch.Tensor, Cn: int, cols: int, name: str) -> int:
+    """Plane stride of src (a frame window, see _frame_window); checks out is a band buffer [T, hs + 2, cols, ldo]."""
+    plane = _frame_window(src, Cn, src.shape[1], name)
+    _need(out, torch.bfloat16, "out")
+    if not out.is_contiguous() or out.dim() != 4 or out.shape[0] != src.shape[1] or out.shape[2] != cols:
+        raise YumeB200Error(f"{name}: out must be a contiguous band buffer [{src.shape[1]}, hs + 2, {cols}, ldo]")
+    return plane
+
+
+def vae_patchify2_bf16_rows(video: torch.Tensor, out: torch.Tensor, r0: int) -> torch.Tensor:
+    """vae_patchify2_bf16_win of the patchified rows r0 - 1 .. r0 + hs (zeros outside the image) into the band buffer out bf16
+    [T, hs + 2, W/2, ldo]; video = whole[:, t0:t0 + T] (f32 [3, T, H, W] frame window of a contiguous video)."""
+    global _launches
+    _, T, H, W = video.shape
+    plane = _rows_reader(video, out, 3, W // 2, "vae_patchify2_bf16_rows")
+    check(_lib.load().yb_vae_patchify2_bf16_rows(video.data_ptr(), plane, out.data_ptr(), out.shape[-1], T, H, W, r0,
+                                                 out.shape[1] - 2, _stream()), "yb_vae_patchify2_bf16_rows")
+    _launches += 1
+    return out
+
+
+def nchw_to_nhwc_bf16_rows(x: torch.Tensor, out: torch.Tensor, r0: int) -> torch.Tensor:
+    """nchw_to_nhwc_bf16_win of rows r0 - 1 .. r0 + hs (zeros outside the image) into the band buffer out bf16 [T, hs + 2, W,
+    ldo]; x = whole[:, t0:t0 + T] (f32 [Cn, T, H, W] frame window of a contiguous video)."""
+    global _launches
+    Cn, T, H, W = x.shape
+    plane = _rows_reader(x, out, Cn, W, "nchw_to_nhwc_bf16_rows")
+    check(_lib.load().yb_nchw_to_nhwc_bf16_rows(x.data_ptr(), plane, out.data_ptr(), out.shape[-1], T, H, W, Cn, r0,
+                                                out.shape[1] - 2, _stream()), "yb_nchw_to_nhwc_bf16_rows")
+    _launches += 1
+    return out

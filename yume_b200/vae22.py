@@ -35,8 +35,7 @@ import torch
 from . import ops
 from ._lib import YumeB200Error
 from .dit import quantize_weight_fp8
-from .vae_rows import RowGroup
-from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _frames_of, _rup, chunk_lengths  # noqa: F401  (chunk_lengths: re-exported)
+from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _rup, chunk_lengths  # noqa: F401  (chunk_lengths: re-exported)
 
 Tensor = torch.Tensor
 
@@ -109,20 +108,6 @@ class WanVaeDecoder(WanVaeEngine):
         b[:zd] = W2 @ mean + sd["conv2.bias"].detach().float()
         self.lin["conv2"] = (w.to(dev, _BF16).contiguous(), b.to(dev))
 
-    def enable_row_parallel(self, group=None) -> "WanVaeDecoder":
-        """Decode on the ranks of `group` (torch.distributed; default the world), each rank its band of rows: rank r of P owns
-        latent rows [floor(rH/P), floor((r+1)H/P)) and every level's rows above them. Every rank still passes the full latent and
-        gets the full clamped video, equal bit for bit to the one-GPU decode: the convs read one halo row of each neighbouring
-        band (exchanged after every norm pass), the mid attention runs on the gathered full frames, and one all-gather at the end
-        of a call assembles the video. A group of one rank keeps the one-GPU path. Call it on every rank; every later decode
-        is then a collective of the group. Raises YumeB200Error without an initialised process group or with precision="fp8"."""
-        if self.precision == "fp8":
-            raise YumeB200Error("enable_row_parallel: the fp8 decode has no row-parallel form; use precision='bf16'")
-        rows = RowGroup(group)
-        self._rows = rows if rows.world > 1 else None
-        self.reset()                                             # kept carries would belong to another band
-        return self
-
     def _input(self, L: Layer, z: Tensor):
         """conv2 (latent de-normalisation folded in) and decoder.conv1 on one chunk of the latent (this rank's band of its rows
         under a row-parallel decode)."""
@@ -183,28 +168,6 @@ class WanVaeDecoder(WanVaeEngine):
                        key=L.name)
         self._write(y, out, dims)
 
-    def _row0(self, rows: int) -> int:
-        """First row of this rank's band at a level whose band has `rows` rows."""
-        r0, hs, _ = self._band
-        return r0 * (rows // hs)
-
-    def _stream(self, src: Tensor, out: Tensor, lengths: Sequence[int], k_in: int, k_out: int, u0: int = 0, *args, **kw):
-        """WanVaeEngine._stream; a row-parallel decode then all-gathers the bands of the frames it wrote."""
-        res = super()._stream(src, out, lengths, k_in, k_out, u0, *args, **kw)
-        t0 = _frames_of(u0, k_out)
-        if self._rows is not None and t0 < out.shape[1]:
-            _, _, H = self._band
-            S = out.shape[2] // H
-            r0, hs, _ = self._band
-            mine = out[:, t0:, r0 * S:(r0 + hs) * S]
-            sizes = [S * h for h in self._rows.sizes(H)]
-            row = 0
-            for r, b in enumerate(self._rows.gather(mine, 2, sizes)):
-                if r != self._rows.rank:
-                    out[:, t0:, row:row + sizes[r]].copy_(b)
-                row += sizes[r]
-        return res
-
     def _t_scale(self) -> int:
         return math.prod(L.ft for L in self.layers if L.kind == "up")
 
@@ -217,12 +180,7 @@ class WanVaeDecoder(WanVaeEngine):
         memory. With resume=True a latent that extends the last call's latent runs only its new frames (WanVaeEngine._resumed)."""
         if z.dim() != 4 or z.shape[0] != self.z_dim:
             raise YumeB200Error(f"expected a latent [{self.z_dim}, T, H, W]")
-        if self._rows is not None:                               # checked on every rank before the first collective
-            H, P = z.shape[2], self._rows.world
-            if H < P:
-                raise YumeB200Error(f"a row-parallel decode on {P} ranks needs at least {P} latent rows, got {H}")
-            r0, r1 = self._rows.band(H)
-            self._band = (r0, r1 - r0, H)
+        self._set_band(z.shape[2])                               # checked on every rank before the first collective
         if self.resume:
             T, H, W = z.shape[1:]
             src = z.to(self.device, _F32).contiguous()

@@ -29,7 +29,7 @@ import torch
 
 from . import ops
 from ._lib import YumeB200Error
-from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _rup
+from .wan_vae import _BF16, _F32, Layer, WanVaeEngine, _attn_bytes, _rup
 
 Tensor = torch.Tensor
 
@@ -105,7 +105,8 @@ def _encoder_tail(c: int, z_dim: int) -> List[Layer]:
 
 class WanVaeEncoder(WanVaeEngine):
     """The encode side of both Wan VAEs: f32 [3, T, H, W] -> mu f32 [z_dim, 1 + (T-1)//4, H/SCALE, W/SCALE]. An engine adds its
-    layer list, SCALE and `_read` (the chunk's video frames into encoder.conv1's input)."""
+    layer list, SCALE and `_read` (the chunk's video frames into encoder.conv1's input, or under a row-parallel encode into the
+    band buffer of its rows)."""
     SCALE: int
 
     @property
@@ -127,11 +128,17 @@ class WanVaeEncoder(WanVaeEngine):
         self.lin["conv1"] = (w.to(dev, _BF16).contiguous(), b.to(dev))
 
     def _input(self, L: Layer, v: Tensor):
-        """encoder.conv1 over its input buffer: carried frames in front, this chunk's frames (patch size L.fs) behind them."""
+        """encoder.conv1 over its input buffer: carried frames in front, this chunk's frames (patch size L.fs) behind them. Under
+        a row-parallel encode the buffer is a band buffer, its rows and both halo rows read straight from the whole video."""
         _, T, H, W = v.shape
         dims = (T, H // L.fs, W // L.fs)
-        x0 = self._hist_buf(L.name, *dims, 64)
-        self._read(v, x0[x0.shape[0] - T:].view(-1, 64))
+        if self._rows is not None:
+            dims = (T, self._band[1] * (dims[1] // self._band[2]), dims[2])
+            x0 = self._hist_buf(L.name, *dims, 64, halo=True)
+            self._read(v, x0[x0.shape[0] - T:])
+        else:
+            x0 = self._hist_buf(L.name, *dims, 64)
+            self._read(v, x0[x0.shape[0] - T:].view(-1, 64))
         return self._conv(L.name, x0, dims, key=L.name), dims
 
     def _resample(self, L: Layer, x: Tensor, dims):
@@ -140,7 +147,10 @@ class WanVaeEncoder(WanVaeEngine):
         p, temporal = L.name, L.ft == 2
         T, H, W = dims
         C = x.shape[1]
-        a = x.view(T, H, W, C) if C % 64 == 0 else self._act(x, dims, None, False)
+        if self._rows is not None:                                 # a band buffer whose row below is the next band's first row
+            a = self._act(x, dims, None, False, halo=True, above=False)
+        else:
+            a = x.view(T, H, W, C) if C % 64 == 0 else self._act(x, dims, None, False)
         _, Ho, Wo = ops.conv_out_dims(T, H, W, (1, 3, 3), 1, 2)
         key = p + ".time_conv"
         if temporal and self._chunk > 0:
@@ -167,11 +177,14 @@ class WanVaeEncoder(WanVaeEngine):
 
     def _head(self, L: Layer, x: Tensor, dims, out: Tensor) -> None:
         """encoder.head + conv1 (mu half) into `out`, this chunk's latent-frame window of the result."""
-        y = self._conv(L.name, self._act(x, dims, "encoder.head.0", True, key=L.name), dims, key=L.name)
+        y = self._conv(L.name, self._act(x, dims, "encoder.head.0", True, key=L.name, halo=True), dims, key=L.name)
         w1, b1 = self.lin["conv1"]
         mu = self._new(y.shape[0], w1.shape[0], dtype=_F32)
         ops.gemm(y, w1, b1, mu, ops.YB_EPI_F32)
-        if self._one_pass:
+        if self._rows is not None:                                 # this rank's rows; _stream gathers the others
+            r0, hs, _ = self._band
+            ops.nhwc_to_nchw_f32_rows(mu, out[:, :, r0:r0 + hs])
+        elif self._one_pass:
             ops.nhwc_to_nchw_f32(mu, out.view(self.z_dim, -1))
         else:
             ops.nhwc_to_nchw_f32_win(mu, out)
@@ -179,6 +192,10 @@ class WanVaeEncoder(WanVaeEngine):
     def _frames(self, video: Tensor) -> Tensor:
         if video.dim() != 4 or video.shape[0] != 3:
             raise YumeB200Error("expected a video [3, T, H, W]")
+        if self._rows is not None:                                 # checked on every rank before the first collective
+            if video.shape[2] % self.SCALE or video.shape[3] % self.SCALE:
+                raise YumeB200Error(f"Wan VAE encode needs H, W divisible by {self.SCALE}")
+            self._set_band(video.shape[2] // self.SCALE)
         keep = 1 + 4 * ((video.shape[1] - 1) // 4)                 # `iter_ = 1 + (t - 1) // 4` chunks of 1, 4, 4, ... (:802-803)
         return video[:, :keep].to(self.device, _F32).contiguous()
 
@@ -209,6 +226,19 @@ class WanVaeEncoder(WanVaeEngine):
         """mu, and the device copy of the video `encode` makes when it is handed one on another device or not contiguous."""
         return 4 * (self.z_dim * (1 + (T - 1) // 4) * (H // self.SCALE) * (W // self.SCALE) + 3 * T * H * W)
 
+    def _band_bytes(self, n: int, T: int, H: int, W: int) -> int:
+        """Upper bound of one rank's device bytes in a row-parallel encode: the largest band in video rows, its halo rows counted
+        at every level as two more latent rows, plus the gathered attention input (padded bands, full frames, the attention's
+        own buffers and the rows kept), the whole video once, and mu with the padded bands of its all-gather."""
+        P, S = self._rows.world, self.SCALE
+        Hl, Wl = H // S, W // S
+        hb = -(-Hl // P)
+        c = next(L for L in self.layers if L.kind == "attn").ci
+        gathered = ((P + 2) * n * hb * Wl + n * Hl * Wl) * c * 2 + _attn_bytes(n, Hl * Wl, c)
+        band = self._chunk_bytes(n, T, (hb + 2) * S, W) - self._fixed_bytes(T, (hb + 2) * S, W)
+        mu = 4 * self.z_dim * (1 + (T - 1) // 4) * Hl * Wl
+        return band + gathered + 4 * 3 * T * H * W + (1 + P) * mu
+
     def plan_chunks(self, T: int, H: int, W: int) -> List[int]:
         """Latent frames per chunk of an encode of T video frames at H x W (see _plan)."""
         return self._plan(1 + (T - 1) // 4, lambda n: self.chunk_bytes(n, T, H, W))
@@ -236,7 +266,9 @@ class Wan22VaeEncoder(WanVaeEncoder):
         super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision, resume)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
-        if self._one_pass:
+        if self._rows is not None:
+            ops.vae_patchify2_bf16_rows(v, dst, self._row0(dst.shape[1] - 2))
+        elif self._one_pass:
             ops.vae_patchify2_bf16(v, dst)
         else:
             ops.vae_patchify2_bf16_win(v, dst)
@@ -264,7 +296,9 @@ class Wan21VaeEncoder(WanVaeEncoder):
         super().__init__(sd, z_dim, layers + _encoder_tail(dims[-1], z_dim), mean, std, device, precision, resume)
 
     def _read(self, v: Tensor, dst: Tensor) -> None:
-        if self._one_pass:
+        if self._rows is not None:
+            ops.nchw_to_nhwc_bf16_rows(v, dst, self._row0(dst.shape[1] - 2))
+        elif self._one_pass:
             ops.nchw_to_nhwc_bf16(v.view(3, -1), dst)
         else:
             ops.nchw_to_nhwc_bf16_win(v, dst)

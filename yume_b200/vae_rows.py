@@ -1,6 +1,7 @@
-"""The transport of a row-parallel Wan VAE decode (WanVaeDecoder.enable_row_parallel): the band partition of the latent's rows,
-the halo-row exchange between neighbouring ranks, the all-gathers of the mid attention's input and of the video, and the
-agreements that keep every rank issuing the same collectives. The kernels of the band forms are include/yume_b200_vae_rows.h.
+"""The transport of a row-parallel Wan VAE decode or encode (WanVaeEngine.enable_row_parallel): the band partition of the
+latent's rows, the halo-row exchange between neighbouring ranks, the all-gathers of the mid attention's input and of the result,
+and the agreements that keep every rank issuing the same collectives. The kernels of the band forms are
+include/yume_b200_vae_rows.h and include/yume_b200_vae_rows_enc.h.
 
 On an NCCL group device tensors go straight through. On any other group (gloo) CPU tensors go straight through and device
 tensors go through host memory, so the same engine runs in the CPU test suite and as several processes sharing one GPU.
@@ -63,6 +64,21 @@ class RowGroup:
         for w in dist.batch_isend_irecv(ops):
             w.wait()
         return tuple(None if t is None else t.to(send.device) for t in recv)
+
+    def from_below(self, send: Tensor) -> Optional[Tensor]:
+        """The one-way exchange of a stride-2 conv, which reads no row above its band: send [2, ...] as in `exchange`, its top row
+        goes to rank - 1. Returns the row below the band (the top row of rank + 1), None on the last rank."""
+        r, P = self.rank, self.world
+        wire = self._wire(send)
+        below = torch.empty_like(wire[0]) if r < P - 1 else None
+        ops = []
+        if r > 0:
+            ops.append(dist.P2POp(dist.isend, wire[0].contiguous(), self._peer(r - 1), self.group))
+        if below is not None:
+            ops.append(dist.P2POp(dist.irecv, below, self._peer(r + 1), self.group))
+        for w in dist.batch_isend_irecv(ops):
+            w.wait()
+        return None if below is None else below.to(send.device)
 
     def gather(self, x: Tensor, dim: int, sizes: Sequence[int]) -> List[Tensor]:
         """All-gather of bands: x is this rank's band (sizes[rank] entries along `dim`); returns every rank's band in rank order

@@ -10,6 +10,7 @@ from typing import Dict, List, NamedTuple, Optional, Sequence, Tuple
 import torch
 
 from ._lib import YumeB200Error
+from .vae_rows import RowGroup
 
 Tensor = torch.Tensor
 _BF16, _F32, _E4M3 = torch.bfloat16, torch.float32, torch.float8_e4m3fn
@@ -56,9 +57,9 @@ class WanVaeEngine:
     # s_w f32 [cop], bias f32 [cop], taps). Their input streams are (e4m3 frames, scale frames) pairs, see _hist_buf.
     conv8: Dict[str, Tuple[Tensor, Tensor, Tensor, tuple]] = {}
     _kept: Optional[_Kept] = None   # resume=True: the state kept from the last call
-    # row-parallel decode (WanVaeDecoder.enable_row_parallel): the RowGroup of the ranks (None: one rank decodes everything) and,
-    # during a call, the band (r0, rows, H) of the latent's H rows this rank owns. dims are then the band's (T, rows, W), and the
-    # input of every conv with kh = 3 is a band buffer with one halo row above and below (include/yume_b200_vae_rows.h).
+    # row-parallel decode or encode (enable_row_parallel): the RowGroup of the ranks (None: one rank runs everything) and, during a
+    # call, the band (r0, rows, H) of the latent's H rows this rank owns. dims are then the band's (T, rows, W), and the input of
+    # every conv with kh = 3 is a band buffer with one halo row above and below (include/yume_b200_vae_rows.h).
     _rows = None
     _band: Tuple[int, int, int] = (0, 0, 0)
 
@@ -76,6 +77,38 @@ class WanVaeEngine:
         mean = torch.zeros(z_dim) if mean is None else mean
         std = torch.ones(z_dim) if std is None else std
         self._repack(sd, mean.detach().to(self.device, _F32), std.detach().to(self.device, _F32))
+
+    def enable_row_parallel(self, group=None) -> "WanVaeEngine":
+        """Run on the ranks of `group` (torch.distributed; default the world), each rank its band of rows: rank r of P owns
+        latent rows [floor(rH/P), floor((r+1)H/P)) and, at every other level, those rows times the level's scale. Every rank
+        still passes the whole input and gets the whole result (a decode's clamped video, an encode's mu), equal bit for bit to
+        the one-GPU call: the convs read one halo row of each neighbouring band (exchanged after every norm pass), the mid
+        attention runs on the gathered full frames, and one all-gather at the end of a call assembles the result. A group of one
+        rank keeps the one-GPU path. Call it on every rank; every later call is then a collective of the group. It drops the
+        state a resuming engine keeps (reset()). Raises YumeB200Error without an initialised process group or with
+        precision="fp8"."""
+        if self.precision == "fp8":
+            raise YumeB200Error("enable_row_parallel: the fp8 decode has no row-parallel form; use precision='bf16'")
+        rows = RowGroup(group)
+        self._rows = rows if rows.world > 1 else None
+        self.reset()                                             # kept carries would belong to another band
+        return self
+
+    def _set_band(self, H: int) -> None:
+        """Under a row-parallel call on H latent rows: this rank's band, or YumeB200Error (raised on every rank, before the first
+        collective) when there are fewer rows than ranks."""
+        if self._rows is None:
+            return
+        P = self._rows.world
+        if H < P:
+            raise YumeB200Error(f"a row-parallel {type(self).__name__} on {P} ranks needs at least {P} latent rows, got {H}")
+        r0, r1 = self._rows.band(H)
+        self._band = (r0, r1 - r0, H)
+
+    def _row0(self, rows: int) -> int:
+        """First row of this rank's band at a level whose band has `rows` rows."""
+        r0, hs, _ = self._band
+        return r0 * (rows // hs)
 
     # ---- weights -------------------------------------------------------------------------------------------
     def _pack_side(self, sd: Dict[str, Tensor], prefixes: Tuple[str, ...], latent_conv: str,
@@ -199,7 +232,9 @@ class WanVaeEngine:
         if out is None:
             To, Ho, Wo = ops.conv_out_dims(T, H, W, taps, stride_t, stride_hw)
             out = self._new(To * Ho * Wo, w.shape[0], dtype=_F32 if epilogue == ops.YB_EPI_F32 else _BF16)
-        if self._rows is not None and a.shape[1] == H + 2:       # a band buffer (_act with halo): the row-halo conv
+        if self._rows is not None and a.shape[1] == H + 2 and stride_hw > 1:    # a band's Resample downsample2d
+            ops.conv3d_rows_down(a, w, b, out, T, H, W, epilogue)
+        elif self._rows is not None and a.shape[1] == H + 2:     # a band buffer (_act with halo): the row-halo conv
             ops.conv3d_rows(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, full_h=self._band[2] * (H // self._band[1]))
         elif h:
             ops.conv3d_causal_hist(a, w, b, out, T, H, W, h, epilogue, res, taps=taps, out_t_mul=out_t_mul,
@@ -210,10 +245,10 @@ class WanVaeEngine:
         return out
 
     def _act(self, x: Tensor, dims, gamma: Optional[str], silu: bool, up: int = 1, key: Optional[str] = None,
-             n: int = 0, conv: Optional[str] = None, halo: bool = False):
+             n: int = 0, conv: Optional[str] = None, halo: bool = False, above: bool = True):
         """The input buffer of the conv `conv` (see _hist_buf): RMS_norm * gamma, SiLU, 2x upsample of x; an e4m3 pair when that
-        conv is one of conv8. halo (a conv with kh = 3) under a row-parallel decode: a band buffer whose halo rows of the T new
-        frames come from the neighbouring ranks."""
+        conv is one of conv8. halo (a conv with kh = 3) under a row-parallel call: a band buffer whose halo rows of the T new
+        frames come from the neighbouring ranks (above=False: only the row below, for the stride-2 Resample conv)."""
         ops = self.ops
         T, H, W = dims
         g = self.gamma[gamma] if gamma else None
@@ -221,7 +256,7 @@ class WanVaeEngine:
             out = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n, halo=True)
             send = self._new(2, T, W * up, out.shape[-1])
             ops.vae_rms_act_rows(x, dims, out[out.shape[0] - T:], g, up, silu, send=send)
-            self._halo(out, T, send)
+            self._halo(out, T, send, above)
             return out
         if conv in self.conv8:
             q, s = self._hist_buf(key, T, H * up, W * up, _rup(x.shape[1], 64), n=n, fp8=True)
@@ -231,14 +266,15 @@ class WanVaeEngine:
         ops.vae_rms_act(x, dims, out[out.shape[0] - T:], g, up, silu)
         return out
 
-    def _halo(self, buf: Tensor, T: int, send: Optional[Tensor] = None) -> None:
+    def _halo(self, buf: Tensor, T: int, send: Optional[Tensor] = None, above: bool = True) -> None:
         """Fill the halo rows of the T new frames of the band buffer `buf` from the neighbouring ranks (zeros at the image's
-        edge). send [2, T, W, Cp]: the band's top and bottom rows of those frames, packed from `buf` when not given."""
+        edge). send [2, T, W, Cp]: the band's top and bottom rows of those frames, packed from `buf` when not given. above=False
+        fills only the row below (the row above is then zeros)."""
         new = buf[buf.shape[0] - T:]
         if send is None:
             send = self._new(2, T, *buf.shape[2:])
             self.ops.vae_rows_pack(new, send)
-        top, bot = self._rows.exchange(send)
+        top, bot = self._rows.exchange(send) if above else (None, self._rows.from_below(send))
         self.ops.vae_rows_unpack(top, bot, new)
 
     def _attention_rows(self, p: str, x: Tensor, dims) -> Tensor:
@@ -345,8 +381,10 @@ class WanVaeEngine:
         """Run latent frames u0 .. u0 + sum(lengths) of `src` in chunks of `lengths` into their frame windows of `out`. u0 > 0
         continues a stream whose carries at latent frame u0 are `carry`: every chunk is then a chunk after the first. keep: the
         last chunk carries as if another followed (a resuming engine). Returns the carries at the end (keep) and those after
-        latent frame `snap` (when a chunk ends there), each a dict the running stream no longer writes into."""
+        latent frame `snap` (when a chunk ends there), each a dict the running stream no longer writes into. A row-parallel call
+        then all-gathers the bands of the frames it wrote."""
         t_in, t_out = _frames_of(u0, k_in), _frames_of(u0, k_out)
+        t0 = t_out
         self._carry = {} if carry is None else dict(carry)
         at_snap = None
         try:
@@ -357,9 +395,24 @@ class WanVaeEngine:
                 t_in, t_out, u0 = t_in + n_in, t_out + n_out, u0 + n
                 if u0 == snap:
                     at_snap = dict(self._carry)                  # _keep replaces carries, never writes into one
-            return (dict(self._carry) if keep else None), at_snap
+            res = (dict(self._carry) if keep else None), at_snap
         finally:
             self._chunk, self._more, self._carry = 0, False, None
+        if self._rows is not None and t0 < out.shape[1]:
+            self._gather_rows(out, t0)
+        return res
+
+    def _gather_rows(self, out: Tensor, t0: int) -> None:
+        """All-gather the row bands of frames t0 .. of the result `out` [C, F, S * H, ...], S its rows per latent row (a decoder's
+        SCALE, 1 for an encoder's mu): every rank wrote its own band, and ends with every band."""
+        r0, hs, H = self._band
+        S = out.shape[2] // H
+        sizes = [S * h for h in self._rows.sizes(H)]
+        row = 0
+        for r, b in enumerate(self._rows.gather(out[:, t0:, r0 * S:(r0 + hs) * S], 2, sizes)):
+            if r != self._rows.rank:
+                out[:, t0:, row:row + sizes[r]].copy_(b)
+            row += sizes[r]
 
     # ---- resuming across calls -----------------------------------------------------------------------------
     def retained_bytes(self) -> int:
@@ -395,8 +448,10 @@ class WanVaeEngine:
         match = torch.empty(2, dtype=torch.int32, device=self.device)
         self.ops.vae_frame_match(kept.src if comparable else None, src, match)
         first, zero = match.tolist()                             # the one synchronisation a resuming call adds
-        if self._rows is not None:                               # every rank resumes from the same snapshot
+        if self._rows is not None:                               # every rank resumes from the same snapshot and forks alike
             first = self._rows.min_int(first if comparable else 0)
+            if fork:
+                zero = self._rows.min_int(zero)
         snaps = kept.snaps if comparable else {}
         P = max((p for p in snaps if p <= first), default=0)
         u0, carry = snaps[P] if P else (0, None)
